@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- Navier2D timesteps/s on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py -- Navier2D timesteps/s on H100 (BASELINE.json metric), one JSON line on stdout.
 
-  python bench.py --gpus N --steps K --warmup W [--config C2|C3|C4|C1] [--impl reference]
+  python bench.py --gpus N --steps K --warmup W [--config C2|C3|C4|C1] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one `Navier2D::update()` (src/navier_stokes/navier.rs:438-466) on synthetic fields:
 constructor defaults, physical fields U(-0.1, 0.1) from numpy default_rng(1/2/3), forward().
 Default workload at every N: BASELINE configs[3] = confined 4097 x 4097 Chebyshev x Chebyshev, Ra 1e9, dt 1e-4
-(the configuration the metric "at 1/2/4/8 B200" and the north-star roofline target are quoted on; it fits one GPU).
+(the configuration the metric "at 1/2/4/8 GPUs" and the north-star roofline target are quoted on; it fits one 80 GB H100).
 --config C2 = configs[1] (1025 x 1025), C3 = configs[2] (periodic 2048 x 1025), C1 = configs[0] (129 x 129).
 
 value  : steps/s with state resident in HBM, CUDA events on the library's stream, max over ranks.
@@ -18,6 +18,10 @@ ops    : ms / transform and ms / solve (the second half of BASELINE.json's metri
 cpu_baseline / --impl reference: the C++/OpenMP restatement of the reference's update() (oracle/cpu_restated.cpp: one
          pass per reference call, lane-parallel, OpenBLAS DGEMM) timed on the host cores (the Rust reference cannot be
          built in this image: no cargo/rustc).
+--dump-outputs DIR: after the timed steps, the state the last timed step computed (the four spectral arrays a caller of
+         update() reads: temp, velx, vely, pres) as DIR/<name>.npy in float64, complex arrays as [..., 2] (real, imaginary);
+         above 2^20 float64 values an array is sampled at fixed flat indices (numpy default_rng(0), sorted) so that the dump
+         stays under 64 MB.  Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 parity_check: 2 steps of a 257 x 129 problem on the same ranks against the numpy oracle (smooth state: 1e-10; white noise:
          max(1e-10, 10 x the oracle's own response to a last-bit change of its input)); parity_check_workload: the
          benchmarked configuration itself against the C++ restatement (1 GPU).
@@ -54,7 +58,7 @@ def config_dict(cfg):
     """`config` of the JSON line: identical in both arms (the repo arm's run details go to `run`)."""
     nx, ny = CONFIGS[cfg][:2]
     return {"workload": workload_name(cfg), "config": cfg,
-            "l2": "per-step working set (~30 arrays x 8N bytes) exceeds the 126 MB L2; no explicit flush" if nx * ny > 600000 else "fits L2"}
+            "l2": "per-step working set (~30 arrays x 8N bytes) exceeds the 50 MB L2 of an H100; no explicit flush" if 30 * 8 * nx * ny > (50 << 20) else "fits L2"}
 
 
 def workload_name(cfg):
@@ -63,7 +67,7 @@ def workload_name(cfg):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -89,6 +93,7 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait(timeout=10)
         sm = sorted(int(r[0]) for r in self.rows if r and r[0].isdigit())
         mx = [int(r[1]) for r in self.rows if len(r) > 1 and r[1].isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -264,6 +269,27 @@ def np_zeros_like_vhat(f):
     return (1.0 / (1.0 + i + j) ** 2).astype(a.dtype)
 
 
+DUMP_VALUES_PER_ARRAY = 1 << 20   # float64 values: 8 MB per array, the four state arrays stay under 64 MB
+
+
+def dump_outputs(state, out_dir, rank):
+    """Write the state arrays as float64 .npy files (complex as [..., 2]); an array of more than DUMP_VALUES_PER_ARRAY
+    float64 values is reduced to the elements at fixed, seeded flat indices, the same for every run of the same configuration."""
+    import numpy as np
+
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in state.items():
+        keep = DUMP_VALUES_PER_ARRAY // (2 if np.iscomplexobj(a) else 1)
+        if a.size > keep:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+            a = np.ascontiguousarray(a).reshape(-1)[idx]
+        if np.iscomplexobj(a):
+            a = np.stack([a.real, a.imag], axis=-1)
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, dtype=np.float64))
+
+
 def parity_small(b2, ctx, dist):
     """2 steps of a 257 x 129 confined problem on the SAME ranks / context as the timed run, gathered and compared with
     the numpy oracle (navier.rs:438-466 / navier_stokes_mpi/navier.rs:497-522).  Cheap; runs before the timing.
@@ -339,9 +365,10 @@ def main():
     ap.add_argument("--ops-multi", action="store_true", help="also time the standalone operators on N > 1 ranks (slab fields)")
     ap.add_argument("--no-parity", action="store_true", help="skip the in-run parity checks (small multi-rank problem; workload vs CPU restatement)")
     ap.add_argument("--mode", type=int, default=1, help="1 fused+graph (default), 3 fused without graph, 0 one pass pair per reference call")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the state of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.config is None:
-        # BASELINE.json quotes its metric "at 1/2/4/8 B200" on configs[3] = confined 4097 x 4097 (C4), which fits one GPU
+        # BASELINE.json quotes its metric "at 1/2/4/8 GPUs" on configs[3] = confined 4097 x 4097 (C4), which fits one GPU
         # and is the size the north-star roofline target is stated on: the same workload at every N, so that the
         # driver's 1 -> 8 series is a strong-scaling series of one problem.  --config C2 / C3 / C1 run the others.
         args.config = "C4"
@@ -405,6 +432,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = float(t.item())
     launches = ctx.launch_count() - l0
+    if args.dump_outputs:
+        dump_outputs(nav.gather_state() if dist is not None else nav.state(), args.dump_outputs, rank)
     ms_per_step = ms / args.steps
     value = 1e3 / ms_per_step
     # keep the same loop running until nvidia-smi (100 ms period) has seen >= 1.5 s of it
@@ -434,11 +463,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:  # noqa: BLE001
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     lane_ms = (ms - gemm_ms) / args.steps
     alg_bytes = 728.0 * N / world   # per GPU
     achieved = alg_bytes / (lane_ms * 1e-3) / 1e9
-    traffic = None   # only a capture of THIS config on ONE GPU counts (profiles/traffic.json is written by tools/gpu_profile.sh)
+    traffic = None   # only a capture of THIS config on ONE GPU counts (profiles/traffic.json: DRAM bytes per step from a profiler capture)
     if world == 1:
         try:
             traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(cfg, {}).get("dram_bytes_per_step")
@@ -471,7 +500,7 @@ def main():
     t_hbm = alg_bytes / (peak * 1e9) * 1e3
     t_gemm = (gemm_flop / (fp64_peak * 1e12) * 1e3) if (fp64_peak and gemm_flop) else 0.0
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                "traffic": traffic, "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 3350 GB/s (H100 SXM data sheet)",
                 "kernel": "lane_kernel (all per-axis passes of one step)", "alg_bytes_per_step": alg_bytes,
                 "lane_ms_per_step": lane_ms, "gemm_ms_per_step": gemm_ms / args.steps,
                 "lane_ms_note": "step time minus the time inside the Poisson GEMMs (FP64-peak-bound, measured with events in a separate un-captured pass)",

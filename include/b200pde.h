@@ -1,4 +1,4 @@
-/* b200pde -- C ABI of the B200-native Navier2D spectral hot path.
+/* b200pde -- C ABI of the H100-native Navier2D spectral hot path.
  *
  * The reference (preiter93/rustpde-mpi) has no FFI: its seam is the Rust trait surface
  * `Space / Field / Solve / Integrate`.  Every entry point below names the reference

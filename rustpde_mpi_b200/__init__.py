@@ -1,7 +1,7 @@
-"""rustpde_mpi_b200 -- B200-native spectral hot path of rustpde's Navier2D / Navier2DMpi.
+"""rustpde_mpi_b200 -- H100-native spectral hot path of rustpde's Navier2D / Navier2DMpi.
 
 Host-side mirror of the reference's Space / Field / Solve / Integrate surface over the C ABI of
-``include/b200pde.h`` (``libb200pde.so``: hand-written sm_100a kernels).  No CPU fallback."""
+``include/b200pde.h`` (``libb200pde.so``: hand-written sm_90a kernels).  No CPU fallback."""
 from .api import (  # noqa: F401
     Context, Space2, Field2, DeviceArray, HholtzAdi, Hholtz, Poisson, Navier2D, integrate,
     chebyshev, cheb_dirichlet, cheb_neumann, cheb_dirichlet_neumann, fourier_r2c, fourier_c2c, poisson_eig, hholtz_eig,

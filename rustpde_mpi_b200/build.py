@@ -1,4 +1,4 @@
-"""Build the CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+"""Build the CUDA library in-tree for sm_90a (H100; nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -22,7 +22,7 @@ def build(force=False, verbose=False):
     if not force and not needs_build():
         return OUT
     tmp = f"{OUT}.{os.getpid()}.tmp"   # build aside and rename: a reader (another rank, a snapshot) never sees a half-written library
-    cmd = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-shared", "-Xcompiler", "-fPIC", "-o", tmp, SRC]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")

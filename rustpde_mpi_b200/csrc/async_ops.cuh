@@ -1,5 +1,5 @@
 // Asynchronous data movement for the lane kernel: TMA tensor copies (global <-> shared), mbarriers,
-// bulk async-groups and named barriers, as thin wrappers over sm_100a PTX.
+// bulk async-groups and named barriers, as thin wrappers over sm_90a PTX.
 //
 // Why: a lane group is a 64-131 KB slab; moving it with per-thread LDG/STG costs registers, issue slots and
 // exposes DRAM latency to every warp.  With TMA one elected thread describes a whole chunk (a box of
@@ -149,7 +149,7 @@ static inline int b2_encode_tmap(const B2TMapDesc& d, B2TMap* out) {
 }
 #else
 // ------------------------------------------------------------------------------------------------
-// sm_100a implementation
+// sm_90a implementation
 // ------------------------------------------------------------------------------------------------
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// b200pde: host side of the B200-native Navier2D spectral hot path + its C ABI.
+// b200pde: host side of the H100-native Navier2D spectral hot path + its C ABI.
 //
 // Mirrors the reference's Space / Field / Solve / Integrate surface (see include/b200pde.h for
 // the file:line of every interface replaced).  Everything numeric runs in lane_kernel.cuh;
@@ -607,7 +607,7 @@ __global__ void k_weighted_rowsum(const double* __restrict__ a, int rows, int co
   out[i] = s;
 }
 
-static int ew_grid(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 148 * 8); }
+static int ew_grid(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132 * 8); }   // 8 CTAs per SM of an H100 SXM
 
 // ------------------------------------------------------------------------------------------------
 // program builder / launcher
@@ -748,8 +748,8 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
   }
   // Generic geometry: a tiled load followed by the composite -> orthonormal stencil (to_ortho: y_j = x_j + s_j x_{j-2}) becomes
   // ONE load that applies the stencil on the fly (LD_STENCIL).  Transform-sized lanes keep the zero-copy load and run the
-  // stencil as a chunk-streaming band op instead (measured on C4: stencil-on-load through the staging slots 20-22k cycles
-  // per lane group, zero-copy load + band_chunk 5.7k + 9.8k; profiles/r02/sweep_*.log).
+  // stencil as a chunk-streaming band op instead (on C4 stencil-on-load through the staging slots took longer per lane group
+  // than the zero-copy load and band_chunk together).
   for (int i = 0; !c.fast && i + 1 < p.nops; i++) {
     LaneOp& lo = p.ops[i]; LaneOp& bo = p.ops[i + 1];
     if (lo.code != OP_LOAD || (lo.i2 & (LD_PLAIN | LD_STENCIL | LD_ACC | LD_MUL)) || bo.code != OP_BAND) continue;
@@ -760,7 +760,7 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
   }
   // Fold a banded mat-vec into the LU solve that consumes it (forward offsets only, same output length; shared
   // coefficient vectors): the solve forms its right-hand side on the fly (lane_fast.cuh, fdma_fast_body<PREBAND>).
-  // Measured: +1.5 % on C2 (E = 8), -2 % on C4 (E = 16, where the extra coefficient streams cost more than the saved
+  // Faster on C2 (E = 8), slower on C4 (E = 16, where the extra coefficient streams cost more than the saved
   // pass), so it is applied to the short-lane instances only.
   if (c.fast && c.E <= 8) {
     for (int i = 0; i + 1 < p.nops; i++) {
@@ -964,7 +964,7 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
   int chw = (int)(room / ((size_t)nwarps * 2) / tile_bytes) - 1;   // one halo tile in front of every slot
   if (const char* e = getenv("B2_CHW")) { int v = atoi(e); if (v >= 2) chw = std::min(chw, v); }
   chw = std::max(2, std::min(chw, std::min(64, c->in_tiles)));
-  if (wbytes > 100 * 1024) chw = std::min(chw, 12);   // long lanes: 12-tile sub-chunks pipeline better than the largest that fit (C4: lane time 8.50 -> 8.27 ms)
+  if (wbytes > 100 * 1024) chw = std::min(chw, 12);   // long lanes: 12-tile sub-chunks pipeline better than the largest that fit (shorter C4 lane time)
   if (nranks > 1) chw = std::max(2, std::min(chw, c->in_tiles / nranks));   // a sub-chunk's tensor-store box never exceeds one owner's rows of the transposed view
   if (c->LN == 2 && (chw % 2 == 0)) chw--;                 // (CHW + 1) tiles of 64 bytes: a multiple of 128
   c->CHW = chw;

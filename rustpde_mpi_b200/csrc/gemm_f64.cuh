@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(G_THREADS, 1) gemm_pb_kernel(const __grid_cons
   };
   // Warp 16 only moves data: it refills a buffer as soon as all 16 compute warps have released it.  (With the copies issued by
   // a compute thread, that thread's warp fell behind by the issue work of every stage, and -- the skew between the warps being
-  // bounded -- all the others waited for it: 4.4 ms of arithmetic took 5.0 ms.)
+  // bounded -- all the others waited for it.)
   if (warp == 16) {
     if (lane == 0 && DBG != 1)
       for (int ks = 0; ks < nks; ks++) {

@@ -16,7 +16,7 @@
 //     access of every operator bank-conflict free in this layout and lets the 4 lanes of a group share
 //     each coefficient / twiddle load (one broadcast request instead of four).
 //
-// sm_100a only.  No CPU fallback, no library calls in here.
+// sm_90a (H100) only.  No CPU fallback, no library calls in here.
 #pragma once
 #ifdef B2_EMU   // tests/emu: the same source compiled for the CPU SIMT emulator (test infrastructure only)
 #include "cuda_emu.h"
@@ -843,6 +843,8 @@ __device__ __noinline__ void op_deriv(const LaneProg& P, const LaneOp& op, doubl
 //   backward: x_i = (x_i - u1_i x_{i+2} - u2_i x_{i+4}) * id_i
 // As pair recurrences: y_p = b_p - fl_p * y_{p-1};  x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p.
 // Each thread reduces its CP pairs to an affine map; maps are combined by a scan across the lane's threads.
+// The four chunk loops stay rolled: the sm_90a build with `#pragma unroll 6` solved wrongly on lanes of 64 points or more
+// (O(1) errors in from_ortho / HholtzAdi; the same source is exact in the CPU emulator and with the loops rolled).
 template <int CP, int LN>
 __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double* __restrict__ W, int gl, int lb, void* scratch) {
   const int TPL = P.TPL, HP = P.LP >> 1;
@@ -869,7 +871,7 @@ __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double
   // ---- forward elimination: y_p = b_p - fl_p y_{p-1} ----
   {
     double2 A = d2(1.0, 1.0), B = zero;
-#pragma unroll 6
+#pragma unroll 1
     for (int t = 0; t < CP; t++) {
       const double2 f = ldg(cfl + base + (size_t)t * stride), b = rd(t);
       B = d2(fma(-f.x, B.x, b.x), fma(-f.y, B.y, b.y));
@@ -878,7 +880,7 @@ __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double
     Aff1::V m; m.d[0] = A.x; m.d[1] = B.x; m.d[2] = A.y; m.d[3] = B.y;
     Aff1::S in = lane_scan_state<Aff1, false, LN>(m, TPL, scratch);
     double2 y = d2(in.d[0], in.d[1]);   // y of the last pair before this chunk (the start state is 0)
-#pragma unroll 6
+#pragma unroll 1
     for (int t = 0; t < CP; t++) {
       const double2 f = ldg(cfl + base + (size_t)t * stride), b = rd(t);
       y = d2(fma(-f.x, y.x, b.x), fma(-f.y, y.y, b.y));
@@ -889,7 +891,7 @@ __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double
   // ---- back substitution: x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p ----
   {
     Aff2::V m = Aff2::identity();
-#pragma unroll 6
+#pragma unroll 1
     for (int t = CP - 1; t >= 0; t--) {
       const size_t k = base + (size_t)t * stride;
       const double2 idv = ldg(cid + k), u1 = ldg(cu1 + k), u2 = nou2 ? zero : ldg(cu2 + k), y = rd(t);
@@ -903,7 +905,7 @@ __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double
     }
     Aff2::S in = lane_scan_state<Aff2, true, LN>(m, TPL, scratch);
     double2 s1 = d2(in.d[0], in.d[2]), s2 = d2(in.d[1], in.d[3]);   // x_{p+1}, x_{p+2} entering the chunk
-#pragma unroll 6
+#pragma unroll 1
     for (int t = CP - 1; t >= 0; t--) {
       const size_t k = base + (size_t)t * stride;
       const double2 idv = ldg(cid + k), u1 = ldg(cu1 + k), u2 = nou2 ? zero : ldg(cu2 + k), y = rd(t);

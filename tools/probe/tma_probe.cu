@@ -3,7 +3,7 @@
 // g = blockIdx.x, blockIdx.x + gridDim.x, ... of a large array and moves every slab HBM -> shared memory (mode L),
 // shared memory -> HBM (mode S) or both, overlapped through two buffers (mode C), with a chosen piece size, number of
 // issuing threads and CTAs per SM.  Prints GB/s and cycles per slab.
-//   build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probe/tma_probe tools/probe/tma_probe.cu
+//   build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probe/tma_probe tools/probe/tma_probe.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
@@ -121,7 +121,7 @@ int main(int argc, char** argv) {
     a.nslabs = l2 ? (int)(((size_t)48 << 20) / slab_b) : nslabs_total;   // l2: a 48 MB working set that stays in L2
     const int reps = l2 ? 12 : 1;
     const size_t smem = 1024 + (size_t)slab_b * (mode == 2 ? 2 : 1);
-    const int grid = 148 * ctas_per_sm;
+    const int grid = 132 * ctas_per_sm;
     if (smem * ctas_per_sm > 226 * 1024) return;
     CK(cudaMemset(cyc, 0, 16));
     probe<<<grid, 512, smem>>>(a);   // warm-up
