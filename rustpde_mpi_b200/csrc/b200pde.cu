@@ -1137,18 +1137,20 @@ static int hholtz_solve(b2_solver* s, const double* in, double* out) {
 // ------------------------------------------------------------------------------------------------
 // FP64 GEMM on the tiled arrays (gemm_f64.cuh): host side
 // ------------------------------------------------------------------------------------------------
-// A (row-major, M x K, leading dimension ld) -> fragment order [slice mt][k stage][k4 step][8-row fragment][lane]:
-// slice mt holds the global rows mt * mstep + row0 + [0, 64); zero outside M x K.
+// A (row-major, M x K, leading dimension ld) -> fragment order [slice mt][k stage][16-row fragment f][k4 slice q][lane][h]
+// = A[16 f + lane / 4 + 8 h][16 ks + 4 q + lane % 4]: the pair h = 0, 1 is the register pair {a[2 (q % 2)], a[2 (q % 2) + 1]}
+// of a thread's mma.m16n8k8 in k8 step q / 2.  Slice mt holds the global rows mt * mstep + row0 + [0, 64); zero outside M x K.
 static std::vector<double> pack_gemm_a(const double* A, int M, int K, int ld, int nmt, int nks, int mstep, int row0) {
   std::vector<double> out((size_t)nmt * nks * G_ACHUNK, 0.0);
   for (int mt = 0; mt < nmt; mt++)
     for (int ks = 0; ks < nks; ks++)
-      for (int kk = 0; kk < G_KK; kk++)
-        for (int mf = 0; mf < 8; mf++)
-          for (int lane = 0; lane < 32; lane++) {
-            const int m = mt * mstep + row0 + 8 * mf + (lane >> 2), k = 4 * G_KK * ks + 4 * kk + (lane & 3);
-            if (m < M && k < K) out[((((size_t)mt * nks + ks) * G_KK + kk) * 8 + mf) * 32 + lane] = A[(size_t)m * ld + k];
-          }
+      for (int f = 0; f < 4; f++)
+        for (int q = 0; q < G_KK; q++)
+          for (int lane = 0; lane < 32; lane++)
+            for (int h = 0; h < 2; h++) {
+              const int m = mt * mstep + row0 + 16 * f + 8 * h + (lane >> 2), k = 4 * G_KK * ks + 4 * q + (lane & 3);
+              if (m < M && k < K) out[(((((size_t)mt * nks + ks) * 4 + f) * G_KK + q) * 32 + lane) * 2 + h] = A[(size_t)m * ld + k];
+            }
   return out;
 }
 // Parity-block product: blocks (Ae: Me x Ke, Ao: Mo x Ko); dense product (Ao == nullptr): one M x K matrix run as two
@@ -1186,7 +1188,8 @@ static int gemm_plan_create(b2_space* sp, GemmPlan* g, const double* Ae, int Me,
 }
 static int gemm_run(b2_ctx* ctx, const GemmPlan& g, const double* B, double* C) {
   static bool attr_set[64] = {false};
-  static const int dbg = getenv("B2_GEMM_DBG") ? atoi(getenv("B2_GEMM_DBG")) : 0;   // measurement only (tools/sweep.py): see gemm_pb_kernel
+  // measurement only (tools/sweep.py): see gemm_pb_kernel; read at every launch so that one process can time several variants
+  const int dbg = getenv("B2_GEMM_DBG") ? atoi(getenv("B2_GEMM_DBG")) : 0;
   if (!attr_set[ctx->device & 63]) {
     CK(cudaFuncSetAttribute(gemm_pb_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     CK(cudaFuncSetAttribute(gemm_pb_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
