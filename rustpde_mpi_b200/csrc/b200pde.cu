@@ -259,6 +259,51 @@ static std::vector<double> pdma_sweep(int n, const std::vector<double> (&d)[7], 
 // natural-order band coefficient vector -> its scan-layout copy (same chunking as the LU coefficients of that axis)
 static std::map<const void*, const void*>& scan_of() { static std::map<const void*, const void*> m; return m; }
 
+// Chunk-map table (LM_* in lane_kernel.cuh) of an LU solve with shared coefficient vectors, keyed by its scan-layout fl vector:
+// the launcher hands the table to the compile-time-geometry solve, which must chunk the lane as the table does (C, TPL).
+struct LuMapRef { const void* table; int C, TPL; };
+static std::map<const void*, LuMapRef>& lumap_of() { static std::map<const void*, LuMapRef> m; return m; }
+
+// Built from the scan-layout vectors (double2 slot [t][q], zero tails), exactly as the device reads them.  Per chunk and parity
+// the back substitution x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p, p = p0 + C - 1 down to p0, is the affine map
+// (x_{p0+C}, x_{p0+C+1}) -> (x_{p0}, x_{p0+1}) with linear part P and translation (sum_t wa_t y_t, sum_t wb_t y_t).
+static std::vector<double> lu_chunk_maps(const std::vector<double>& fl, const std::vector<double>& id, const std::vector<double>& u1,
+                                         const std::vector<double>* u2, int C, int TPL) {
+  const int NS = LM_CHUNK * C + LMC_N;
+  std::vector<double> o((size_t)2 * NS * TPL, 0.0);
+  std::vector<long double> wa(C), wb(C);
+  for (int q = 0; q < TPL; q++)
+    for (int h = 0; h < 2; h++) {
+      auto in = [&](const std::vector<double>& v, int t) -> long double { return v[((size_t)t * TPL + q) * 2 + h]; };
+      auto out = [&](int s) -> double& { return o[((size_t)s * TPL + q) * 2 + h]; };
+      long double A = 1.0L, P00 = 1.0L, P01 = 0.0L, P10 = 0.0L, P11 = 1.0L;
+      for (int t = 0; t < C; t++) {
+        const long double u2t = u2 ? in(*u2, t) : 0.0L;
+        out(LM_FL * C + t) = (double)in(fl, t); out(LM_ID * C + t) = (double)in(id, t);
+        out(LM_U1 * C + t) = (double)(in(u1, t) * in(id, t)); out(LM_U2 * C + t) = (double)(u2t * in(id, t));
+        A *= -in(fl, t);
+      }
+      for (int t = C - 1; t >= 0; t--) {   // compose pair t onto the map of pairs t+1 .. C-1
+        const long double m0 = -in(u1, t) * in(id, t), m1 = -(u2 ? in(*u2, t) : 0.0L) * in(id, t);
+        for (int k = t + 1; k < C; k++) { const long double a = wa[k]; wa[k] = m0 * a + m1 * wb[k]; wb[k] = a; }
+        wa[t] = in(id, t); wb[t] = 0.0L;
+        const long double r0 = m0 * P00 + m1 * P10, r1 = m0 * P01 + m1 * P11;
+        P10 = P00; P11 = P01; P00 = r0; P01 = r1;
+      }
+      for (int t = 0; t < C; t++) { out(LM_WA * C + t) = (double)wa[t]; out(LM_WB * C + t) = (double)wb[t]; }
+      out(LM_CHUNK * C + LMC_A) = (double)A;
+      out(LM_CHUNK * C + LMC_P + 0) = (double)P00; out(LM_CHUNK * C + LMC_P + 1) = (double)P01;
+      out(LM_CHUNK * C + LMC_P + 2) = (double)P10; out(LM_CHUNK * C + LMC_P + 3) = (double)P11;
+    }
+  return o;
+}
+static int upload_lu_maps(const void* fl_key, const std::vector<double>& fl, const std::vector<double>& id, const std::vector<double>& u1,
+                          const std::vector<double>* u2, int C, int TPL, DVecD* table) {
+  RET(table->upload(lu_chunk_maps(fl, id, u1, u2, C, TPL)));
+  lumap_of()[fl_key] = LuMapRef{table->d, C, TPL};
+  return B2_OK;
+}
+
 struct Base1 {
   int kind = 0, n = 0, m = 0;
   bool cheb = false, composite = false;   // composite: ChebDirichlet / ChebNeumann (stencil at even offsets: pair-structured lane operators)
@@ -272,6 +317,7 @@ struct Base1 {
   DVecD d_dfwd, d_dbwd; bool dense_tr = false;       // transform sizes the FFT core does not handle: dense matrices (OP_DENSE)
   DVecD d_ca, d_cb, d_pent; int pent_L = 0;            // cdn: stencil vectors, packed PdmaPlus2 LU of S^T S (from_ortho)
   DVecD d_s2_sc, d_bd_sc, d_bu1_sc, d_bu2_sc, d_sten2s_sc;   // scan-layout copies for band ops folded into an LU solve (see run_pass)
+  DVecD d_tmap;                                               // chunk-map table of the from_ortho solve (lumap_of)
 
   // B2 = laplace_inv (SURVEY 8a row G); pv(i, off) = (laplace_inv_eye . laplace_inv)[i, i+off]
   double pv(int i, int off) const {
@@ -331,7 +377,8 @@ struct Base1 {
   void release() {
     const void* keys[] = {d_bd.d, d_bu1.d, d_bu2.d, d_s2.d, d_sten2s.d};
     for (auto k : keys) if (k) scan_of().erase(k);
-    DVecD* all[] = {&d_sten2, &d_sten2s, &d_s2, &d_tfl, &d_tid, &d_tu1, &d_bd, &d_bu1, &d_bu2, &d_tw, &d_tw2, &d_isin, &d_s2_sc, &d_bd_sc, &d_bu1_sc, &d_bu2_sc, &d_sten2s_sc, &d_ca, &d_cb, &d_pent, &d_dfwd, &d_dbwd};
+    if (d_tfl.d) lumap_of().erase(d_tfl.d);
+    DVecD* all[] = {&d_sten2, &d_sten2s, &d_s2, &d_tfl, &d_tid, &d_tu1, &d_bd, &d_bu1, &d_bu2, &d_tw, &d_tw2, &d_isin, &d_s2_sc, &d_bd_sc, &d_bu1_sc, &d_bu2_sc, &d_sten2s_sc, &d_ca, &d_cb, &d_pent, &d_dfwd, &d_dbwd, &d_tmap};
     for (auto* v : all) v->release();
   }
 };
@@ -387,7 +434,9 @@ int Base1::init(int C, int TPL) {
     }
     LuVecs lu = sweep(t);
     lu.fl.resize(L, 0.0); lu.id.resize(L, 0.0); lu.u1.resize(L, 0.0);
-    RET(d_tfl.upload(scan_layout(lu.fl))); RET(d_tid.upload(scan_layout(lu.id))); RET(d_tu1.upload(scan_layout(lu.u1)));
+    const std::vector<double> tfl = scan_layout(lu.fl), tid = scan_layout(lu.id), tu1 = scan_layout(lu.u1);
+    RET(d_tfl.upload(tfl)); RET(d_tid.upload(tid)); RET(d_tu1.upload(tu1));
+    RET(upload_lu_maps(d_tfl.d, tfl, tid, tu1, nullptr, C, TPL, &d_tmap));
     // MatVecFdma of the preconditioner pinv (src/solver/matvec.rs:177-203)
     std::vector<double> bd(L, 0.0), bu1(L, 0.0), bu2(L, 0.0);
     for (int i = 0; i < m; i++) {
@@ -518,6 +567,7 @@ struct b2_solver {
   int type = 0;  // 0 hholtz_adi, 1 poisson
   // per axis: banded LU (Chebyshev) or reciprocal diagonal (Fourier)
   DVecD fl[2], id[2], u1[2], u2[2], sd[2], pd[2];   // pd: packed PdmaPlus2 LU (ChebDirichletNeumann axis)
+  DVecD lm[2];                                       // chunk-map tables of the banded LU solves (lumap_of)
   int pd_L[2] = {0, 0};
   // poisson
   bool dense = false;
@@ -761,7 +811,8 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
   // Fold a banded mat-vec into the LU solve that consumes it (forward offsets only, same output length; shared
   // coefficient vectors): the solve forms its right-hand side on the fly (lane_fast.cuh, fdma_fast_body<PREBAND>).
   // Faster on C2 (E = 8), slower on C4 (E = 16, where the extra coefficient streams cost more than the saved
-  // pass), so it is applied to the short-lane instances only.
+  // pass; still 0.14 ms per step slower with the chunk-map solve, H100 SXM at 400 W), so it is applied to the short-lane
+  // instances only.
   if (c.fast && c.E <= 8) {
     for (int i = 0; i + 1 < p.nops; i++) {
       LaneOp& bo = p.ops[i]; LaneOp& fo = p.ops[i + 1];
@@ -778,6 +829,15 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
       if (!ok) continue;
       bo.code = OP_PREBAND; bo.p0 = sc[0]; bo.p1 = sc[1]; bo.p2 = sc[2]; fo.i2 |= FD_PREBAND;
     }
+  }
+  // LU solves with shared coefficient vectors run on their chunk-map table on transform-sized lanes (fdma_fast_body)
+  for (int i = 0; c.fast && i < p.nops; i++) {
+    LaneOp& fo = p.ops[i];
+    if (fo.code != OP_FDMA || (fo.i2 & FD_PERLANE)) continue;
+    const auto it = lumap_of().find(fo.p0);
+    if (it == lumap_of().end() || it->second.C != c.C || it->second.TPL != c.TPL)
+      return fail(B2_ERR_ARG, "LU solve without a chunk-map table for this lane layout");
+    fo.p0 = it->second.table;
   }
   // Remaining banded mat-vecs on transform-sized lanes run in chunk-streaming form (band_chunk: one read and one write
   // traversal of the lane group): pair offsets {0, +1, +2} or {0, -1}, vector coefficients through their scan-layout copies.
@@ -1077,10 +1137,10 @@ static int op_forward_ortho_dealias(b2_space* sp, const double* phys, double* or
 // ------------------------------------------------------------------------------------------------
 // solvers
 // ------------------------------------------------------------------------------------------------
-static int upload_lu(const LuVecs& lu, const Base1& b, DVecD* fl, DVecD* id, DVecD* u1, DVecD* u2) {
-  RET(fl->upload(b.scan_layout(lu.fl))); RET(id->upload(b.scan_layout(lu.id)));
-  RET(u1->upload(b.scan_layout(lu.u1))); RET(u2->upload(b.scan_layout(lu.u2)));
-  return B2_OK;
+static int upload_lu(const LuVecs& lu, const Base1& b, DVecD* fl, DVecD* id, DVecD* u1, DVecD* u2, DVecD* map) {
+  const std::vector<double> sfl = b.scan_layout(lu.fl), sid = b.scan_layout(lu.id), su1 = b.scan_layout(lu.u1), su2 = b.scan_layout(lu.u2);
+  RET(fl->upload(sfl)); RET(id->upload(sid)); RET(u1->upload(su1)); RET(u2->upload(su2));
+  return upload_lu_maps(fl->d, sfl, sid, su1, &su2, b.lay_C, b.lay_TPL, map);
 }
 
 static int hholtz_create(b2_space* sp, double c0, double c1, b2_solver** out) {
@@ -1098,7 +1158,7 @@ static int hholtz_create(b2_space* sp, double c0, double c1, b2_solver** out) {
         mat.up1[i] = a.up1[i] - bm.up1[i] * c[ax];
         mat.up2[i] = a.up2[i] - bm.up2[i] * c[ax];
       }
-      RET(upload_lu(sweep(mat), b, &s->fl[ax], &s->id[ax], &s->u1[ax], &s->u2[ax]));
+      RET(upload_lu(sweep(mat), b, &s->fl[ax], &s->id[ax], &s->u1[ax], &s->u2[ax], &s->lm[ax]));
     } else if (b.cdn) {  // PdmaPlus2::from_matrix(mat), src/solver/hholtz_adi.rs:64
       std::vector<double> d[7];
       b.cdn_hholtz_diags(c[ax], d);
@@ -1808,7 +1868,10 @@ int b2_hholtz_create(const b2_field* f, double c0, double c1, const double* lam,
 }
 int b2_solver_destroy(b2_solver* s) {
   if (!s) return B2_OK;
-  for (int ax = 0; ax < 2; ax++) { s->fl[ax].release(); s->id[ax].release(); s->u1[ax].release(); s->u2[ax].release(); s->sd[ax].release(); s->pd[ax].release(); }
+  for (int ax = 0; ax < 2; ax++) {
+    if (s->fl[ax].d) lumap_of().erase(s->fl[ax].d);
+    s->fl[ax].release(); s->id[ax].release(); s->u1[ax].release(); s->u2[ax].release(); s->sd[ax].release(); s->pd[ax].release(); s->lm[ax].release();
+  }
   s->pfl.release(); s->pid.release(); s->pu1.release(); s->pu2.release();
   s->qfl.release(); s->qid.release(); s->qu1.release(); s->qu2.release();
   for (GemmPlan* g : {&s->gf, &s->gb}) { g->A[0].release(); g->A[1].release(); }

@@ -400,17 +400,24 @@ __device__ __noinline__ void deriv_fast(const LaneProg& P, const LaneOp& op, dou
   }
 }
 
-// LU solve (see op_fdma).  PERLANE: coefficient arrays [group][t][q][lane of 4] instead of shared [t][q].
+// LU solve (see op_fdma).  PERLANE: coefficient arrays [group][t][q][lane of 4] instead of shared [t][q].  Shared vectors come
+// as the chunk-map table (LM_*): the forward chunk map needs no product of coefficients, the back-substitution chunk map is a
+// weighted sum of the chunk's y (2 FMA per pair and parity instead of composing a 2x2 affine map per pair), and the solve does
+// not multiply by id.  The per-lane arrays stream from HBM (one set per lane), where a table of 6 vectors instead of 4 would
+// cost more traffic than the arithmetic it saves, so they keep the composing form.
 template <int E, int LN, int TPL, bool PERLANE, bool PREBAND>
 __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& op, double* __restrict__ W, int gl, int lb, void* scratch) {
   constexpr int CP = E + 1, CS = PERLANE ? 4 * TPL : TPL;
+  constexpr bool MAPS = !PERLANE;
   const int HP = P.LP >> 1;
   const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
   const int n = op.i0;
   double2* w2 = reinterpret_cast<double2*>(W) + 2 * l;
   const size_t cb = PERLANE ? ((size_t)gl * CP * TPL + q) * 4 + lb + l : (size_t)q;
-  const double2* __restrict__ cfl = (const double2*)op.p0 + cb; const double2* __restrict__ cid = (const double2*)op.p1 + cb;
-  const double2* __restrict__ cu1 = (const double2*)op.p2 + cb; const double2* __restrict__ cu2 = (const double2*)op.p3 + cb;
+  const double2* __restrict__ cfl = (const double2*)op.p0 + cb;   // MAPS: the table, slot LM_FL = 0
+  const double2* __restrict__ cid = MAPS ? cfl + LM_ID * CP * TPL : (const double2*)op.p1 + cb;
+  const double2* __restrict__ cu1 = MAPS ? cfl + LM_U1 * CP * TPL : (const double2*)op.p2 + cb;
+  const double2* __restrict__ cu2 = MAPS ? cfl + LM_U2 * CP * TPL : (const double2*)op.p3 + cb;
   const bool nou2 = op.i2 & FD_NOU2;
   const double2 zero = d2(0.0, 0.0);
   const int p0 = q * CP;
@@ -426,6 +433,11 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
     return v;
   };
   PhaseClock pc(P.prof);
+  // MAPS: translation of the back-substitution chunk map = the weighted sums of the chunk's y, accumulated as the forward pass
+  // produces y (no separate pass over the chunk)
+  double2 ta = zero, tb = zero;
+  const double2* __restrict__ cwa = cfl + LM_WA * CP * TPL;
+  const double2* __restrict__ cwb = cfl + LM_WB * CP * TPL;
   // ---- forward elimination: y_p = b_p - fl_p y_{p-1} ----
   {
     double2 A = d2(1.0, 1.0), B = zero;
@@ -463,7 +475,7 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
         if (t < tmax) w2[ca.at(t)] = b;
         const double2 f = ldg(cfl + t * CS);
         B = d2(fma(-f.x, B.x, b.x), fma(-f.y, B.y, b.y));
-        A = d2(-f.x * A.x, -f.y * A.y);
+        if constexpr (!MAPS) A = d2(-f.x * A.x, -f.y * A.y);
         x0 = x1; x1 = x2;
       }
     } else if (interior) {
@@ -471,16 +483,17 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
       for (int t = 0; t < CP; t++) {
         const double2 f = ldg(cfl + t * CS), b = w2[ca.at(t)];
         B = d2(fma(-f.x, B.x, b.x), fma(-f.y, B.y, b.y));
-        A = d2(-f.x * A.x, -f.y * A.y);
+        if constexpr (!MAPS) A = d2(-f.x * A.x, -f.y * A.y);
       }
     } else {
 #pragma unroll
       for (int t = 0; t < CP; t++) {
         const double2 f = ldg(cfl + t * CS), b = rdm(t);
         B = d2(fma(-f.x, B.x, b.x), fma(-f.y, B.y, b.y));
-        A = d2(-f.x * A.x, -f.y * A.y);
+        if constexpr (!MAPS) A = d2(-f.x * A.x, -f.y * A.y);
       }
     }
+    if constexpr (MAPS) A = ldg(cfl + (LM_CHUNK * CP + LMC_A) * TPL);
     pc.mark(16);
     Aff1::V m; m.d[0] = A.x; m.d[1] = B.x; m.d[2] = A.y; m.d[3] = B.y;
     Aff1::S in = lane_scan_state<Aff1, false, LN>(m, TPL, scratch);
@@ -492,6 +505,7 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
         const double2 f = ldg(cfl + t * CS), b = w2[ca.at(t)];
         y = d2(fma(-f.x, y.x, b.x), fma(-f.y, y.y, b.y));
         w2[ca.at(t)] = y;
+        if constexpr (MAPS) { ta = d2fma(ldg(cwa + t * TPL), y, ta); tb = d2fma(ldg(cwb + t * TPL), y, tb); }
       }
     } else {
 #pragma unroll
@@ -499,6 +513,12 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
         const double2 f = ldg(cfl + t * CS), b = rdm(t);
         y = d2(fma(-f.x, y.x, b.x), fma(-f.y, y.y, b.y));
         if (t < tmax) w2[ca.at(t)] = y;
+        if constexpr (MAPS) {   // the y the back substitution reads: zero outside [0, n) and beyond the lane
+          double2 v = (t < tmax) ? y : zero;
+          if (t >= tx) v.x = 0.0;
+          if (t >= ty) v.y = 0.0;
+          ta = d2fma(ldg(cwa + t * TPL), v, ta); tb = d2fma(ldg(cwb + t * TPL), v, tb);
+        }
       }
     }
   }
@@ -507,22 +527,29 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
   // ---- back substitution: x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p ----
   {
     Aff2::V m = Aff2::identity();
-    auto compose = [&](int t, double2 y) {   // compose pair t onto the chunk map; state = (x_{p+1}, x_{p+2}) per component
-      const double2 idv = ldg(cid + t * CS), u1 = ldg(cu1 + t * CS), u2 = nou2 ? zero : ldg(cu2 + t * CS);
-      const double2 m0 = d2(-u1.x * idv.x, -u1.y * idv.y), m1 = d2(-u2.x * idv.x, -u2.y * idv.y), g0 = d2(y.x * idv.x, y.y * idv.y);
-      double* Mx = m.d;
-      double r0 = m0.x * Mx[0] + m1.x * Mx[2], r1 = m0.x * Mx[1] + m1.x * Mx[3], rp = m0.x * Mx[4] + m1.x * Mx[5] + g0.x;
-      Mx[2] = Mx[0]; Mx[3] = Mx[1]; Mx[5] = Mx[4]; Mx[0] = r0; Mx[1] = r1; Mx[4] = rp;
-      Mx = m.d + 6;
-      r0 = m0.y * Mx[0] + m1.y * Mx[2]; r1 = m0.y * Mx[1] + m1.y * Mx[3]; rp = m0.y * Mx[4] + m1.y * Mx[5] + g0.y;
-      Mx[2] = Mx[0]; Mx[3] = Mx[1]; Mx[5] = Mx[4]; Mx[0] = r0; Mx[1] = r1; Mx[4] = rp;
-    };
-    if (interior) {
-#pragma unroll
-      for (int t = CP - 1; t >= 0; t--) compose(t, w2[ca.at(t)]);
+    if constexpr (MAPS) {   // linear part of the chunk map from the table, translation from the forward pass
+      const double2* __restrict__ cP = cfl + (LM_CHUNK * CP + LMC_P) * TPL;
+      const double2 P00 = ldg(cP), P01 = ldg(cP + TPL), P10 = ldg(cP + 2 * TPL), P11 = ldg(cP + 3 * TPL);
+      m.d[0] = P00.x; m.d[1] = P01.x; m.d[2] = P10.x; m.d[3] = P11.x; m.d[4] = ta.x; m.d[5] = tb.x;
+      m.d[6] = P00.y; m.d[7] = P01.y; m.d[8] = P10.y; m.d[9] = P11.y; m.d[10] = ta.y; m.d[11] = tb.y;
     } else {
+      auto compose = [&](int t, double2 y) {   // compose pair t onto the chunk map; state = (x_{p+1}, x_{p+2}) per component
+        const double2 idv = ldg(cid + t * CS), u1 = ldg(cu1 + t * CS), u2 = nou2 ? zero : ldg(cu2 + t * CS);
+        const double2 m0 = d2(-u1.x * idv.x, -u1.y * idv.y), m1 = d2(-u2.x * idv.x, -u2.y * idv.y), g0 = d2(y.x * idv.x, y.y * idv.y);
+        double* Mx = m.d;
+        double r0 = m0.x * Mx[0] + m1.x * Mx[2], r1 = m0.x * Mx[1] + m1.x * Mx[3], rp = m0.x * Mx[4] + m1.x * Mx[5] + g0.x;
+        Mx[2] = Mx[0]; Mx[3] = Mx[1]; Mx[5] = Mx[4]; Mx[0] = r0; Mx[1] = r1; Mx[4] = rp;
+        Mx = m.d + 6;
+        r0 = m0.y * Mx[0] + m1.y * Mx[2]; r1 = m0.y * Mx[1] + m1.y * Mx[3]; rp = m0.y * Mx[4] + m1.y * Mx[5] + g0.y;
+        Mx[2] = Mx[0]; Mx[3] = Mx[1]; Mx[5] = Mx[4]; Mx[0] = r0; Mx[1] = r1; Mx[4] = rp;
+      };
+      if (interior) {
 #pragma unroll
-      for (int t = CP - 1; t >= 0; t--) compose(t, rdm(t));
+        for (int t = CP - 1; t >= 0; t--) compose(t, w2[ca.at(t)]);
+      } else {
+#pragma unroll
+        for (int t = CP - 1; t >= 0; t--) compose(t, rdm(t));
+      }
     }
     pc.mark(19);
     Aff2::S in = lane_scan_state<Aff2, true, LN>(m, TPL, scratch);
@@ -530,7 +557,8 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
     double2 s1 = d2(in.d[0], in.d[2]), s2 = d2(in.d[1], in.d[3]);   // x_{p+1}, x_{p+2} entering the chunk
     auto solve = [&](int t, double2 y) -> double2 {
       const double2 idv = ldg(cid + t * CS), u1 = ldg(cu1 + t * CS), u2 = nou2 ? zero : ldg(cu2 + t * CS);
-      const double2 x = d2((y.x - u1.x * s1.x - u2.x * s2.x) * idv.x, (y.y - u1.y * s1.y - u2.y * s2.y) * idv.y);
+      const double2 x = MAPS ? d2(fma(-u1.x, s1.x, fma(-u2.x, s2.x, idv.x * y.x)), fma(-u1.y, s1.y, fma(-u2.y, s2.y, idv.y * y.y)))   // u1, u2 times id
+                             : d2((y.x - u1.x * s1.x - u2.x * s2.x) * idv.x, (y.y - u1.y * s1.y - u2.y * s2.y) * idv.y);
       s2 = s1; s1 = x;
       return x;
     };

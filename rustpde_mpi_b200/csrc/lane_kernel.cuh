@@ -41,7 +41,8 @@ enum LaneOpCode {
   OP_STORE = 2,    // dst = [dst +] a * W            i0=len  i2=flags(ST_*)       p0=dst  (p1=peer table)
   OP_BAND = 3,     // y_i = sum_m c_m[i] x_{i+o_m}   i0=len_out i1=packed offs i2=len_in  p0..p2 coef (null = 1, i1 byte=127: unused)
   OP_DERIV = 4,    // Chebyshev d/dx of i0 coeffs, i1 times, times a
-  OP_FDMA = 5,     // banded LU solve (fwd elim + back subst)  i0=len i2=flags(FD_*) p0=fl p1=inv_dia p2=u1 p3=u2
+  OP_FDMA = 5,     // banded LU solve (fwd elim + back subst)  i0=len i2=flags(FD_*) p0=fl p1=inv_dia p2=u1 p3=u2 (fast geometry,
+                   //   shared vectors: p0 = chunk-map table, LM_*)
   OP_DCT = 6,      // Chebyshev transform, i0=n (=N+1), i1: 0 fwd (values->coeffs) 1 bwd   p0=tw p1=tw2 p2=isin
   OP_RFFT = 7,     // Fourier r2c/c2r, i0=n, i1: 0 fwd 1 bwd                              p0=tw p1=tw2
   OP_FDIFF = 8,    // interleaved complex modes: c_k *= (i k)^{i1} * a,  i0 = number of modes, i2 = n for FFT-ordered modes (c2c) else 0
@@ -75,6 +76,15 @@ enum { ST_ACC = 1, ST_PLAIN = 2, ST_TRANS = 8, ST_PEER = 16,
                              // (operand of the eigen-transform GEMM, whose contraction runs over the rows); p1 = peer table
 enum { FD_PERLANE = 1, FD_NOU2 = 2,
        FD_PREBAND = 4 };   // the right-hand side is the banded mat-vec described by the preceding OP_PREBAND op
+// Chunk maps of an LU solve with shared coefficient vectors (set by the launcher on transform-sized lanes: OP_FDMA p0 = the
+// table, see fdma_fast_body).  Everything in it depends on the coefficients only, so the host computes it once.  double2 slot
+// [s][q] of the thread that owns pairs q*CP + t (both parities), s = LM_x * CP + t for the per-pair entries:
+//   LM_FL: fl   LM_ID: id   LM_U1: u1 * id   LM_U2: u2 * id
+//   LM_WA, LM_WB: weight of y_t in x_{p0} and x_{p0+1} of the chunk's back-substitution map (entered with zero state)
+// and LM_CHUNK * CP + LMC_x for the per-chunk entries: LMC_A = product of -fl over the chunk (linear part of the forward map),
+// LMC_P .. LMC_P + 3 = P00 P01 P10 P11 (linear part of the back-substitution map, Aff2 order).
+enum { LM_FL = 0, LM_ID, LM_U1, LM_U2, LM_WA, LM_WB, LM_CHUNK };
+enum { LMC_A = 0, LMC_P = 1, LMC_N = 5 };
 
 struct LaneOp {
   int code, i0, i1, i2;
