@@ -72,6 +72,11 @@ int b2_space_destroy(b2_space* sp);
 /* shape_physical / shape_spectral / ortho shape; spectral & ortho of r2c spaces are complex */
 int b2_space_shape(const b2_space* sp, int shape_kind, int* rows, int* cols, int* is_complex);
 int b2_space_coords(const b2_space* sp, int axis, double* x_host /* n values */);
+/* lane-kernel layout of the passes along one direction (orient 0: lanes along axis 1, 1: lanes along axis 0), host only:
+   out[6] = {E (FFT points per thread), LN (lanes per CTA), TPL (threads per lane), fast (1: compile-time-geometry instance
+   (E, LN, TPL), 0: the generic instance of (E, LN)), CHW (tiles per copy sub-chunk), NT (threads per CTA)}.  A test and
+   diagnostic query with no reference counterpart: it lets a test prove which kernel instance a space reaches. */
+int b2_space_layout(const b2_space* sp, int orient, int* out /* 6 values */);
 
 /* ---- device arrays (the `Array2<T>` values that flow between Field and Solve calls) ---- */
 int b2_array_create(b2_space* sp, int shape_kind, b2_array** out);

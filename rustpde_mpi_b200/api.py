@@ -186,6 +186,14 @@ class Space2:
             out.append(x)
         return out
 
+    def layout(self, orient):
+        """Lane-kernel layout of the passes with lanes along axis 1 (orient 0) or axis 0 (orient 1): {E, LN, TPL, fast, CHW,
+        NT}; fast = the compile-time-geometry instance (E, LN, TPL) runs, else the generic one of (E, LN).  A test and
+        diagnostic query; the reference has no counterpart."""
+        out = (C.c_int * 6)()
+        check(lib().b2_space_layout(self._h, orient, out))
+        return dict(zip(("E", "LN", "TPL", "fast", "CHW", "NT"), (int(v) for v in out)))
+
 
 def _release(fn, handle):
     """Destroy a native object from close()/__del__: never raises (interpreter shutdown, already-destroyed context)."""

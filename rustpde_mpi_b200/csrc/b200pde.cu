@@ -1659,6 +1659,13 @@ int b2_space_coords(const b2_space* sp, int axis, double* x) {
   for (int j = 0; j < b.n; j++) x[j] = b.cheb ? -std::cos(PI * j / (b.n - 1)) : 2.0 * PI * j / b.n;
   return B2_OK;
 }
+int b2_space_layout(const b2_space* sp, int orient, int* out) {
+  if (!sp || !out) return fail(B2_ERR_ARG, "b2_space_layout: null");
+  if (orient < 0 || orient > 1) return fail(B2_ERR_ARG, "orient");
+  const PassCfg& c = sp->cfg[orient];
+  out[0] = c.E; out[1] = c.LN; out[2] = c.TPL; out[3] = c.fast ? 1 : 0; out[4] = c.CHW; out[5] = c.NT;
+  return B2_OK;
+}
 
 int b2_array_create(b2_space* sp, int shape_kind, b2_array** out) {
   int r, c;

@@ -523,7 +523,9 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
     }
   }
   pc.mark(18);
-  // every thread only touched its own chunk: no barrier needed before the back substitution
+  // every thread only touched its own chunk of W: no barrier needed before the back substitution.  The scan scratch needs none
+  // either: the back substitution's warp totals never overlap the entry states a slower warp may still be reading from the
+  // forward scan (lane_scan_state)
   // ---- back substitution: x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p ----
   {
     Aff2::V m = Aff2::identity();

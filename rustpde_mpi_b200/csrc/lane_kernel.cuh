@@ -33,7 +33,8 @@
 #define B2_MAXPEERS 8
 #define B2_MAXPST 6     // transposing stores per program that can go to peer GPUs through tensor maps
 #define B2_BARBYTES 512  // mbarriers at the start of dynamic shared memory: dfull + 2 per warp
-#define B2_SCRATCH 8192  // bytes of scan scratch (16 warps x 4 lanes x (Aff2 map + state))
+#define B2_SCRATCH 8192  // bytes of scan scratch: 16 warps x 4 lanes x (Aff2 map + Aff2 state); entry states at one fixed offset
+                         // behind the largest warp totals (see lane_scan_state)
 #define B2_PROGCOPY 2048 // shared-memory copy of the program header + ops (everything of LaneProg in front of tm[])
 
 enum LaneOpCode {
@@ -327,11 +328,20 @@ struct Aff2 {
 // SUFFIX: q' > q, highest applied first) applied to the zero state.  Threads of a lane sit LN apart in a warp
 // (32/LN of them per warp); warp totals go through shared memory and ONE thread per lane runs the short
 // serial recurrence over the warps (vector recurrence only -- no matrix products on the critical path).
-// scratch: >= 16 warps * LN lanes * (V + S).  All threads of the CTA must call.
+// scratch: [warp totals tot: 16 warps * LN lanes * V][entry states ent at 16 * LN * sizeof(Aff2::V), the same offset for
+// every map type: 16 * LN * S].  All threads of the CTA must call.
+// Scratch invariant (callers run scans back to back without a barrier in between, e.g. the two scans of an LU solve):
+// no scan's tot overlaps any scan's ent.  A warp reads its ent[w] after the scan's last barrier and nothing waits for that
+// read, so a fast warp may already be writing the NEXT scan's tot while a slow one still reads ent.  ent itself is only
+// written between the two barriers of a scan (by tid < LN), and every thread has read the previous scan's ent before it
+// arrives at the first of them.
 template <class M, bool SUFFIX, int LN>
 __device__ __forceinline__ typename M::S lane_scan_state(typename M::V mine, int TPL, void* scratch) {
   typedef typename M::V V;
   typedef typename M::S S;
+  static_assert(sizeof(V) <= sizeof(Aff2::V), "warp totals would overlap the entry states of another scan");
+  static_assert(sizeof(S) <= sizeof(Aff2::S), "entry states would run past the scan scratch");
+  static_assert(16 * 4 * (sizeof(Aff2::V) + sizeof(Aff2::S)) <= B2_SCRATCH, "scan scratch too small");
   constexpr int QW = 32 / LN;                    // threads of one lane inside a warp
   const int tid = threadIdx.x, l = tid & (LN - 1);
   const int qi = (tid & 31) >> Lay<LN>::LOG;     // position inside the warp's segment of the lane
@@ -350,7 +360,7 @@ __device__ __forceinline__ typename M::S lane_scan_state(typename M::V mine, int
   if (TPL <= QW) return M::apply(exc, M::zero());
   const int nw = TPL / QW, w = tid >> 5;
   V* tot = reinterpret_cast<V*>(scratch);                  // [warp][lane] warp totals
-  S* ent = reinterpret_cast<S*>(tot + 16 * LN);            // [warp][lane] state entering the warp
+  S* ent = reinterpret_cast<S*>(static_cast<char*>(scratch) + 16 * LN * sizeof(Aff2::V));   // [warp][lane] state entering the warp
   if (SUFFIX ? (qi == 0) : (qi == QW - 1)) tot[w * LN + l] = inc;
   __syncthreads();
   if (tid < LN) {
@@ -897,7 +907,9 @@ __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double
       if (p0 + t < HP) w2[Lay<LN>::pix(p0 + t)] = y;
     }
   }
-  // every thread only touched its own chunk: no barrier needed before the back substitution
+  // every thread only touched its own chunk of W: no barrier needed before the back substitution.  The scan scratch needs none
+  // either: the back substitution's warp totals never overlap the entry states a slower warp may still be reading from the
+  // forward scan (lane_scan_state)
   // ---- back substitution: x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p ----
   {
     Aff2::V m = Aff2::identity();

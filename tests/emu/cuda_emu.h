@@ -171,7 +171,34 @@ inline double shfl(double v, int src_lane) {
 #define blockDim emu::g_blockDim
 #define gridDim emu::g_gridDim
 
-static inline void __syncthreads() { emu::block().bar.wait(); }
+namespace emu {
+// B2_EMU_SKEW_US=<us>[,rev|fwd]: a deterministic race schedule.  After every block barrier warp w sleeps before it resumes:
+// rev (default) (nwarps - 1 - w) * us, so low warps resume last; fwd w * us, so high warps resume last.  A read that some
+// warp makes after a barrier and that nothing orders against another warp's later write then loses the race every time.
+// Unset: no sleep (the normal emulator).  One-warp blocks never sleep.
+struct Skew { long us = 0; bool fwd = false; };
+inline const Skew& skew() {
+  static const Skew s = [] {
+    Skew r;
+    if (const char* e = getenv("B2_EMU_SKEW_US")) {
+      r.us = std::max(0L, atol(e));
+      const char* c = strchr(e, ',');
+      r.fwd = c && strcmp(c + 1, "fwd") == 0;
+    }
+    return r;
+  }();
+  return s;
+}
+}  // namespace emu
+static inline void __syncthreads() {
+  emu::block().bar.wait();
+  const emu::Skew& s = emu::skew();
+  if (s.us > 0) {
+    const int nw = (emu::g_blockDim.x + 31) / 32, w = emu::t_threadIdx.x / 32;
+    const long d = s.fwd ? w : nw - 1 - w;
+    if (d > 0) std::this_thread::sleep_for(std::chrono::microseconds(d * s.us));
+  }
+}
 static inline void __syncwarp() { emu::block().warps[threadIdx.x / 32].bar.wait(); }
 static inline double __shfl_up_sync(unsigned, double v, int d, int width = 32) {
   const int lane = threadIdx.x % 32;

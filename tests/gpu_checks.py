@@ -155,8 +155,12 @@ def navier_errors(no, ng):
     return out
 
 
-def check_navier(nx, ny, steps, periodic=False, ra=1e5, dt=0.01, init="modes", bc="rbc"):
+def check_navier(nx, ny, steps, periodic=False, ra=1e5, dt=0.01, init="modes", bc="rbc", mode=None):
+    """``mode``: the step schedule of the CUDA side (Navier2D.set_mode: bit 0 fused, bit 1 no CUDA-graph replay, bit 2 no
+    parallel branches); None keeps the default (fused, branches, graph replay)."""
     no, ng = make_navier_pair(nx, ny, ra, 1.0, dt, 1.0, periodic, init, bc)
+    if mode is not None:
+        ng.set_mode(mode)
     for _ in range(steps):
         no.update()
     ng.update(steps)

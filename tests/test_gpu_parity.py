@@ -24,23 +24,31 @@ def test_field_ops(sp, op):
     assert getattr(g, "check_" + op)(*sp) < g.TOL
 
 
-@pytest.mark.parametrize("sp", SPACES[:7], ids=IDS[:7])
+# lanes that run the E = 16 instances at their natural size: (16,4,64) along axis 0, (16,4,128) along axis 1, r2c (16,4,64)
+E16 = [(1, 2049, 2, 65), (2, 65, 1, 4097), (4, 2048, 2, 65)]
+E16_IDS = ["-".join(f"{g.KIND_NAME[s[i]]}{s[i+1]}" for i in (0, 2)) for s in E16]
+
+
+@pytest.mark.parametrize("sp", SPACES[:7] + E16, ids=IDS[:7] + E16_IDS)
 @pytest.mark.parametrize("deriv", [(1, 0), (0, 1), (2, 0), (0, 2), (1, 1)])
 def test_gradient(sp, deriv):
     assert g.check_gradient(*sp, deriv) < g.TOL
 
 
-@pytest.mark.parametrize("sp", [s for s in SPACES if s[0] != 0 and s[2] != 0][:6])
+@pytest.mark.parametrize("sp", [s for s in SPACES if s[0] != 0 and s[2] != 0][:6] + E16)
 def test_hholtz_adi(sp):
     assert g.check_hholtz(*sp) < g.TOL
 
 
-@pytest.mark.parametrize("sp", [(2, 65, 2, 65), (2, 129, 2, 65), (2, 257, 2, 257), (4, 64, 2, 65), (4, 256, 2, 129)])
+# (2,57,2,129) / (1,63,1,129): parity blocks of 28 / 27 rows and a one-tile last column block of the eigen-transform GEMM
+@pytest.mark.parametrize("sp", [(2, 65, 2, 65), (2, 129, 2, 65), (2, 257, 2, 257), (4, 64, 2, 65), (4, 256, 2, 129),
+                                (2, 57, 2, 129), (1, 63, 1, 129)] + E16)
 def test_poisson(sp):
     assert g.check_poisson(*sp) < g.TOL
 
 
-@pytest.mark.parametrize("sp", [(1, 65, 1, 65), (2, 129, 1, 65), (1, 257, 2, 257), (4, 64, 1, 65), (4, 256, 2, 129)])
+@pytest.mark.parametrize("sp", [(1, 65, 1, 65), (2, 129, 1, 65), (1, 257, 2, 257), (4, 64, 1, 65), (4, 256, 2, 129),
+                                (1, 57, 2, 129), (2, 63, 1, 129)])
 def test_hholtz_tensor(sp):
     """Hholtz (src/solver/hholtz.rs:66-101): the eigendecomposition form of the Helmholtz solve (own FP64 GEMM path)."""
     assert g.check_hholtz_tensor(*sp) < g.TOL

@@ -122,13 +122,19 @@ def test_c4_random_state_cpp_checker():
 
 
 LONG = [(1, 65, 0, 8193), (4, 8192, 1, 65), (0, 8193, 1, 65), (2, 65, 2, 8193)]
+LONG_IDS = ["-".join(f"{g.KIND_NAME[s[i]]}{s[i+1]}" for i in (0, 2)) for s in LONG]
+# HholtzAdi needs a base with boundary conditions (or Fourier) on both axes
+LONG_CASES = [(sp, op, f"{op}-{sid}") for op in ["roundtrip_layout", "forward", "backward", "to_ortho", "from_ortho", "hholtz", "gradient"]
+              for sp, sid in zip(LONG, LONG_IDS) if op != "hholtz" or 0 not in (sp[0], sp[2])]
 
 
-@pytest.mark.parametrize("sp", LONG, ids=["-".join(f"{g.KIND_NAME[s[i]]}{s[i+1]}" for i in (0, 2)) for s in LONG])
-@pytest.mark.parametrize("op", ["roundtrip_layout", "forward", "backward", "to_ortho", "from_ortho"])
+@pytest.mark.parametrize("sp,op", [c[:2] for c in LONG_CASES], ids=[c[2] for c in LONG_CASES])
 def test_long_lane_ops(sp, op):
-    """8192 / 8193-point lanes (the C5 / 8193^2 kernel instances)."""
-    e = getattr(g, "check_" + op)(*sp)
+    """8192 / 8193-point lanes (the C5 / 8193^2 kernel instances): transforms, derivatives and HholtzAdi."""
+    if op == "gradient":
+        e = max(g.check_gradient(*sp, d) for d in ((1, 0), (0, 1), (2, 0), (0, 2)))
+    else:
+        e = getattr(g, "check_" + op)(*sp)
     assert e == 0.0 if op == "roundtrip_layout" else e < TOL
 
 
