@@ -256,13 +256,40 @@ static std::vector<double> pdma_sweep(int n, const std::vector<double> (&d)[7], 
   return out;
 }
 
-// natural-order band coefficient vector -> its scan-layout copy (same chunking as the LU coefficients of that axis)
-static std::map<const void*, const void*>& scan_of() { static std::map<const void*, const void*> m; return m; }
+// pair/scan order of a coefficient vector for the chunking (C, TPL): double2 slot [t*TPL + q] = (v[2p], v[2p+1]), p = q*C + t
+static std::vector<double> scan_layout(const std::vector<double>& v, int C, int TPL) {
+  std::vector<double> o((size_t)2 * C * TPL, 0.0);
+  for (int q = 0; q < TPL; q++)
+    for (int t = 0; t < C; t++) {
+      const size_t p = (size_t)q * C + t, k = (size_t)t * TPL + q;
+      if (2 * p < v.size()) o[2 * k] = v[2 * p];
+      if (2 * p + 1 < v.size()) o[2 * k + 1] = v[2 * p + 1];
+    }
+  return o;
+}
 
-// Chunk-map table (LM_* in lane_kernel.cuh) of an LU solve with shared coefficient vectors, keyed by its scan-layout fl vector:
-// the launcher hands the table to the compile-time-geometry solve, which must chunk the lane as the table does (C, TPL).
-struct LuMapRef { const void* table; int C, TPL; };
-static std::map<const void*, LuMapRef>& lumap_of() { static std::map<const void*, LuMapRef> m; return m; }
+// Coefficient vector of a banded mat-vec: natural order (OP_BAND, generic geometry) and its scan-layout copy for the chunking
+// (C, TPL) it was built for (OP_BANDC / OP_PREBAND, transform-sized lanes).
+struct BandVec {
+  DVecD nat, scan;
+  int C = 0, TPL = 0;
+  int upload(const std::vector<double>& v, int C_, int TPL_) {
+    C = C_; TPL = TPL_;
+    RET(nat.upload(v));
+    return scan.upload(scan_layout(v, C, TPL));
+  }
+  void release() { nat.release(); scan.release(); }
+};
+
+// LU coefficients of a banded solve (OP_FDMA) in scan layout for the chunking (C, TPL) they were built for: one set shared by
+// every lane, with the chunk-map table that the compile-time-geometry solve runs on (map), or one set per lane (perlane, the
+// Poisson per-row LU: [lane group][t][q][lane]).  u2 absent: FD_NOU2.
+struct LuDev {
+  DVecD fl, id, u1, u2, map;
+  int C = 0, TPL = 0;
+  bool perlane = false;
+  void release() { fl.release(); id.release(); u1.release(); u2.release(); map.release(); }
+};
 
 // Built from the scan-layout vectors (double2 slot [t][q], zero tails), exactly as the device reads them.  Per chunk and parity
 // the back substitution x_p = (y_p - u1_p x_{p+1} - u2_p x_{p+2}) id_p, p = p0 + C - 1 down to p0, is the affine map
@@ -297,11 +324,14 @@ static std::vector<double> lu_chunk_maps(const std::vector<double>& fl, const st
     }
   return o;
 }
-static int upload_lu_maps(const void* fl_key, const std::vector<double>& fl, const std::vector<double>& id, const std::vector<double>& u1,
-                          const std::vector<double>* u2, int C, int TPL, DVecD* table) {
-  RET(table->upload(lu_chunk_maps(fl, id, u1, u2, C, TPL)));
-  lumap_of()[fl_key] = LuMapRef{table->d, C, TPL};
-  return B2_OK;
+// shared-vector LU (with u2 or without) for the chunking (C, TPL), with its chunk-map table
+static int upload_lu(const LuVecs& lu, bool with_u2, int C, int TPL, LuDev* out) {
+  const std::vector<double> sfl = scan_layout(lu.fl, C, TPL), sid = scan_layout(lu.id, C, TPL), su1 = scan_layout(lu.u1, C, TPL);
+  const std::vector<double> su2 = scan_layout(lu.u2, C, TPL);
+  out->C = C; out->TPL = TPL;
+  RET(out->fl.upload(sfl)); RET(out->id.upload(sid)); RET(out->u1.upload(su1));
+  if (with_u2) RET(out->u2.upload(su2));
+  return out->map.upload(lu_chunk_maps(sfl, sid, su1, with_u2 ? &su2 : nullptr, C, TPL));
 }
 
 struct Base1 {
@@ -312,12 +342,13 @@ struct Base1 {
   int rows_phys = 0, rows_spec = 0, rows_ortho = 0;  // real rows along this axis (complex => 2 per mode)
   int N = 0;                                          // transform size (n-1 Chebyshev, n Fourier)
   std::vector<double> s2;                             // stencil: ortho_k = c_k + s2[k-2] c_{k-2}
-  DVecD d_sten2, d_sten2s, d_s2, d_tfl, d_tid, d_tu1, d_bd, d_bu1, d_bu2, d_tw, d_tw2, d_isin;
+  BandVec bsten, bs2;                                 // composite: stencil of to_ortho (bsten[j] = s2[j-2]), S^T of from_ortho
+  BandVec bd, bu1, bu2;                               // composite / cdn: MatVecFdma of the preconditioner pinv
+  LuDev tlu;                                          // composite: from_ortho solve (S^T S) c = S^T o
+  DVecD d_tw, d_tw2, d_isin;
   std::vector<double> ca, cb;                         // cdn stencil: ortho_k = c_k + ca[k-1] c_{k-1} + cb[k-2] c_{k-2}
   DVecD d_dfwd, d_dbwd; bool dense_tr = false;       // transform sizes the FFT core does not handle: dense matrices (OP_DENSE)
   DVecD d_ca, d_cb, d_pent; int pent_L = 0;            // cdn: stencil vectors, packed PdmaPlus2 LU of S^T S (from_ortho)
-  DVecD d_s2_sc, d_bd_sc, d_bu1_sc, d_bu2_sc, d_sten2s_sc;   // scan-layout copies for band ops folded into an LU solve (see run_pass)
-  DVecD d_tmap;                                               // chunk-map table of the from_ortho solve (lumap_of)
 
   // B2 = laplace_inv (SURVEY 8a row G); pv(i, off) = (laplace_inv_eye . laplace_inv)[i, i+off]
   double pv(int i, int off) const {
@@ -363,23 +394,10 @@ struct Base1 {
   int init_host(int kind_, int n_);
   int init(int C, int TPL);   // device vectors; (C, TPL) = chunking of the passes whose lanes run along this axis
   int lay_C = 1, lay_TPL = 1;
-  // pair/scan order of a coefficient vector: double2 slot [t*TPL + q] = (v[2p], v[2p+1]), p = q*CP + t
-  std::vector<double> scan_layout(const std::vector<double>& v) const {
-    std::vector<double> o((size_t)2 * lay_C * lay_TPL, 0.0);
-    for (int q = 0; q < lay_TPL; q++)
-      for (int t = 0; t < lay_C; t++) {
-        const size_t p = (size_t)q * lay_C + t, k = (size_t)t * lay_TPL + q;
-        if (2 * p < v.size()) o[2 * k] = v[2 * p];
-        if (2 * p + 1 < v.size()) o[2 * k + 1] = v[2 * p + 1];
-      }
-    return o;
-  }
   void release() {
-    const void* keys[] = {d_bd.d, d_bu1.d, d_bu2.d, d_s2.d, d_sten2s.d};
-    for (auto k : keys) if (k) scan_of().erase(k);
-    if (d_tfl.d) lumap_of().erase(d_tfl.d);
-    DVecD* all[] = {&d_sten2, &d_sten2s, &d_s2, &d_tfl, &d_tid, &d_tu1, &d_bd, &d_bu1, &d_bu2, &d_tw, &d_tw2, &d_isin, &d_s2_sc, &d_bd_sc, &d_bu1_sc, &d_bu2_sc, &d_sten2s_sc, &d_ca, &d_cb, &d_pent, &d_dfwd, &d_dbwd, &d_tmap};
-    for (auto* v : all) v->release();
+    for (BandVec* v : {&bsten, &bs2, &bd, &bu1, &bu2}) v->release();
+    tlu.release();
+    for (DVecD* v : {&d_tw, &d_tw2, &d_isin, &d_ca, &d_cb, &d_pent, &d_dfwd, &d_dbwd}) v->release();
   }
 };
 
@@ -425,29 +443,23 @@ int Base1::init(int C, int TPL) {
     std::vector<double> sten2(L, 0.0), s2v(L, 0.0);
     for (int i = 2; i < n; i++) sten2[i] = s2[i - 2];
     for (int k = 0; k < m; k++) s2v[k] = s2[k];
-    RET(d_sten2.upload(sten2)); RET(d_sten2s.upload(sten2)); RET(d_s2.upload(s2v));   // banded mat-vec coefficients: natural order
+    RET(bsten.upload(sten2, C, TPL)); RET(bs2.upload(s2v, C, TPL));
     // from_ortho: (S^T S) c = S^T o, tridiagonal at offsets (-2,0,2) (SURVEY A.2)
     Diags t(m);
     for (int k = 0; k < m; k++) {
       t.dia[k] = 1.0 + s2[k] * s2[k];
       if (k + 2 < m) { t.low[k] = s2[k]; t.up1[k] = s2[k]; }
     }
-    LuVecs lu = sweep(t);
-    lu.fl.resize(L, 0.0); lu.id.resize(L, 0.0); lu.u1.resize(L, 0.0);
-    const std::vector<double> tfl = scan_layout(lu.fl), tid = scan_layout(lu.id), tu1 = scan_layout(lu.u1);
-    RET(d_tfl.upload(tfl)); RET(d_tid.upload(tid)); RET(d_tu1.upload(tu1));
-    RET(upload_lu_maps(d_tfl.d, tfl, tid, tu1, nullptr, C, TPL, &d_tmap));
-    // MatVecFdma of the preconditioner pinv (src/solver/matvec.rs:177-203)
-    std::vector<double> bd(L, 0.0), bu1(L, 0.0), bu2(L, 0.0);
+    RET(upload_lu(sweep(t), false, C, TPL, &tlu));
+  }
+  if (composite || cdn) {   // MatVecFdma of the preconditioner pinv (src/solver/matvec.rs:177-203), the same for every composite base
+    std::vector<double> vd(L, 0.0), vu1(L, 0.0), vu2(L, 0.0);
     for (int i = 0; i < m; i++) {
-      bd[i] = pv(i, 0);
-      if (i < m - 2) bu1[i] = pv(i, 2);
-      if (i < m - 4) bu2[i] = pv(i, 4);
+      vd[i] = pv(i, 0);
+      if (i < m - 2) vu1[i] = pv(i, 2);
+      if (i < m - 4) vu2[i] = pv(i, 4);
     }
-    RET(d_bd.upload(bd)); RET(d_bu1.upload(bu1)); RET(d_bu2.upload(bu2));
-    RET(d_bd_sc.upload(scan_layout(bd))); RET(d_bu1_sc.upload(scan_layout(bu1))); RET(d_bu2_sc.upload(scan_layout(bu2))); RET(d_s2_sc.upload(scan_layout(s2v)));
-    scan_of()[d_bd.d] = d_bd_sc.d; scan_of()[d_bu1.d] = d_bu1_sc.d; scan_of()[d_bu2.d] = d_bu2_sc.d; scan_of()[d_s2.d] = d_s2_sc.d;
-    RET(d_sten2s_sc.upload(scan_layout(sten2))); scan_of()[d_sten2s.d] = d_sten2s_sc.d;
+    RET(bd.upload(vd, C, TPL)); RET(bu1.upload(vu1, C, TPL)); RET(bu2.upload(vu2, C, TPL));
   }
   if (cdn) {
     std::vector<double> a(L, 0.0), b(L, 0.0);
@@ -463,16 +475,6 @@ int Base1::init(int C, int TPL) {
     }
     pent_L = L;
     RET(d_pent.upload(pdma_sweep(m, d, L)));
-    // MatVecFdma of the preconditioner pinv (the same for every composite base)
-    std::vector<double> bd(L, 0.0), bu1(L, 0.0), bu2(L, 0.0);
-    for (int i = 0; i < m; i++) {
-      bd[i] = pv(i, 0);
-      if (i < m - 2) bu1[i] = pv(i, 2);
-      if (i < m - 4) bu2[i] = pv(i, 4);
-    }
-    RET(d_bd.upload(bd)); RET(d_bu1.upload(bu1)); RET(d_bu2.upload(bu2));
-    RET(d_bd_sc.upload(scan_layout(bd))); RET(d_bu1_sc.upload(scan_layout(bu1))); RET(d_bu2_sc.upload(scan_layout(bu2)));
-    scan_of()[d_bd.d] = d_bd_sc.d; scan_of()[d_bu1.d] = d_bu1_sc.d; scan_of()[d_bu2.d] = d_bu2_sc.d;
   }
   // transform tables (only when the size is one the FFT core handles)
   if (is_pow2(N) && N >= 64) {
@@ -566,18 +568,18 @@ struct b2_solver {
   b2_space* sp = nullptr;
   int type = 0;  // 0 hholtz_adi, 1 poisson
   // per axis: banded LU (Chebyshev) or reciprocal diagonal (Fourier)
-  DVecD fl[2], id[2], u1[2], u2[2], sd[2], pd[2];   // pd: packed PdmaPlus2 LU (ChebDirichletNeumann axis)
-  DVecD lm[2];                                       // chunk-map tables of the banded LU solves (lumap_of)
+  LuDev lu[2];
+  DVecD sd[2], pd[2];   // pd: packed PdmaPlus2 LU (ChebDirichletNeumann axis)
   int pd_L[2] = {0, 0};
   // poisson
   bool dense = false;
   int m0 = 0;
-  DVecD pfl, pid, pu1, pu2; // per-lane LU in scan layout
+  LuDev pl;                 // per-lane LU
   // parity blocks: the eigenvectors couple indices of equal parity only, so with the modes grouped by parity class both
   // GEMMs split into two half-size GEMMs (half the flops)
   bool blocks = false;
   int ce = 0, co = 0;       // even / odd indices (= modes of the even / odd class)
-  DVecD qfl, qid, qu1, qu2; // per-lane LU for the parity-grouped mode order
+  LuDev ql;                 // per-lane LU for the parity-grouped mode order
   // own FP64 GEMM on the tiled arrays (gemm_f64.cuh): forward (x -> eigenmodes) and backward products
   GemmPlan gf, gb;
   bool own_gemm = false;
@@ -664,10 +666,22 @@ static int ew_grid(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132
 // ------------------------------------------------------------------------------------------------
 static int pack_offs(int o0, int o1, int o2) { return (o0 & 0xff) | ((o1 & 0xff) << 8) | ((o2 & 0xff) << 16); }
 
+// A lane program for the passes of one space and orientation (orient 0: lanes along axis 1; orient 1: lanes along axis 0).
+// Every op is emitted in the form that the pass's kernel instance runs: the chunk-streaming band ops, the folded mat-vec and
+// the chunk-map solves on transform-sized lanes (c.fast), the natural-order forms and stencil-on-load on the generic instance.
 struct Prog {
   LaneProg p;
+  b2_space* sp;
+  int orient;
+  const PassCfg& c;
   int err = B2_OK;
-  Prog() { memset(&p, 0, sizeof(p)); }
+  Prog(b2_space* sp_, int orient_) : sp(sp_), orient(orient_), c(sp_->cfg[orient_]) { memset(&p, 0, sizeof(p)); }
+  // coefficients in scan layout must be chunked as the lanes of this pass
+  bool chunked(int C, int TPL, const char* what) {
+    if (C == c.C && TPL == c.TPL) return true;
+    err = fail(B2_ERR_ARG, std::string(what) + " built for another lane layout");
+    return false;
+  }
   LaneOp* add(int code) {
     if (p.nops >= B2_MAXOPS) { err = fail(B2_ERR_ARG, "lane program too long"); return &p.ops[B2_MAXOPS - 1]; }
     LaneOp* o = &p.ops[p.nops++];
@@ -677,12 +691,37 @@ struct Prog {
   }
   void load(const double* src, int len, double a = 1.0, int flags = 0, int i1 = 0) { LaneOp* o = add(OP_LOAD); o->p0 = src; o->i0 = len; o->a = a; o->i2 = flags; o->i1 = i1; }
   void store(double* dst, int len, int flags, double a = 1.0, int i1 = 0) { LaneOp* o = add(OP_STORE); o->p0 = dst; o->i0 = len; o->a = a; o->i2 = flags; o->i1 = i1; }
-  void band(int len_out, int len_in, int o0, const double* c0, int o1, const double* c1, int o2 = 127, const double* c2 = nullptr) {
-    LaneOp* o = add(OP_BAND); o->i0 = len_out; o->i2 = len_in; o->i1 = pack_offs(o0, o1, o2); o->p0 = c0; o->p1 = c1; o->p2 = c2;
+  // Banded mat-vec y_i = k0_i x_i + k1_i x_{i+o1} + k2_i x_{i+4}: o1 = +2, or -2 for the to_ortho stencil; k0 null = 1, k2
+  // null = no term.  Transform-sized lanes run it in chunk-streaming form (OP_BANDC, band_chunk: one read and one write
+  // traversal of the lane group) on the scan-layout copies, or fold it into the LU solve emitted next (OP_PREBAND).
+  void band(int len_out, int len_in, const BandVec* k0, int o1, const BandVec& k1, const BandVec* k2 = nullptr, bool fold = false) {
+    const BandVec* k[3] = {k0, &k1, k2};
+    LaneOp* o = add(OP_BAND); o->i0 = len_out; o->i2 = len_in; o->i1 = pack_offs(0, o1, k2 ? 4 : 127);
+    const void** cp[3] = {&o->p0, &o->p1, &o->p2};
+    for (int m = 0; m < 3; m++) {
+      if (!k[m]) continue;
+      if (c.fast && !chunked(k[m]->C, k[m]->TPL, "band coefficients")) return;
+      *cp[m] = c.fast ? k[m]->scan.d : k[m]->nat.d;
+    }
+    if (!c.fast) return;
+    if (fold) { o->code = OP_PREBAND; return; }
+    o->code = OP_BANDC;   // term flags: 1 unit coefficient, 2 vector (band_chunk)
+    o->i1 = (o1 < 0 ? 1 : 0) | ((k0 ? 2 : 1) << 2) | (2 << 4) | ((k2 ? 2 : 0) << 6);
   }
   void deriv(int n, int times, double scale) { LaneOp* o = add(OP_DERIV); o->i0 = n; o->i1 = times; o->a = scale; }
-  void fdma(int len, const double* fl, const double* id, const double* u1, const double* u2, int flags) {
-    LaneOp* o = add(OP_FDMA); o->i0 = len; o->i2 = flags; o->p0 = fl; o->p1 = id; o->p2 = u1; o->p3 = u2;
+  // LU solve; shared vectors run on their chunk-map table on transform-sized lanes (fdma_fast_body)
+  void fdma(int len, const LuDev& lu, int flags = 0) {
+    if (!chunked(lu.C, lu.TPL, "LU solve")) return;
+    LaneOp* o = add(OP_FDMA); o->i0 = len; o->i2 = flags | (lu.perlane ? FD_PERLANE : 0) | (lu.u2.d ? 0 : FD_NOU2);
+    o->p0 = c.fast && !lu.perlane ? lu.map.d : lu.fl.d; o->p1 = lu.id.d; o->p2 = lu.u1.d; o->p3 = lu.u2.d;
+  }
+  // LU solve with shared vectors of the mat-vec (k0, k1 at +2, k2 at +4) of W.  On E <= 8 transform-sized lanes the solve forms
+  // that right-hand side itself from the OP_PREBAND op just before it (fdma_fast_body reads it there).  On E = 16 the extra
+  // coefficient streams cost more than the saved pass (0.14 ms per step slower on C4, H100 SXM at 400 W), so it stays OP_BANDC.
+  void band_solve(int len, int len_in, const BandVec* k0, const BandVec& k1, const BandVec* k2, const LuDev& lu) {
+    const bool fold = c.fast && c.E <= 8;
+    band(len, len_in, k0, 2, k1, k2, fold);
+    fdma(len, lu, fold ? FD_PREBAND : 0);
   }
   void dense(int n_out, int n_in, const double* M) { LaneOp* o = add(OP_DENSE); o->i0 = n_out; o->i1 = n_in; o->p0 = M; }
   void dct(const Base1& b, int mode) {
@@ -703,17 +742,24 @@ struct Prog {
   void sten3(int len_out, int mode, const Base1& b) { LaneOp* o = add(OP_STEN3); o->i0 = len_out; o->i1 = mode; o->p0 = b.d_ca.d; o->p1 = b.d_cb.d; }
   void pdma(int n, const double* packed, int L) { LaneOp* o = add(OP_PDMA); o->i0 = n; o->i1 = L; o->p0 = packed; }
   int to_ortho(const Base1& b) {
-    if (b.composite) { band(b.n, b.m, 0, nullptr, -2, b.d_sten2s.d); return b.n; }
+    if (b.composite) {
+      // Generic geometry: a plain load of the composite coefficients applies the stencil y_j = x_j + s_j x_{j-2} on the fly
+      // (LD_STENCIL).  Transform-sized lanes keep the zero-copy load and stream the stencil (on C4 stencil-on-load through the
+      // staging slots took longer per lane group than the zero-copy load and band_chunk together).
+      LaneOp* lo = p.nops ? &p.ops[p.nops - 1] : nullptr;
+      if (!c.fast && lo && lo->code == OP_LOAD && !(lo->i2 & (LD_PLAIN | LD_STENCIL | LD_ACC | LD_MUL)) && lo->i0 == b.m) {
+        lo->i2 |= LD_STENCIL; lo->p1 = b.bsten.nat.d; lo->i0 = b.n;
+      } else {
+        band(b.n, b.m, nullptr, -2, b.bsten);
+      }
+      return b.n;
+    }
     if (b.cdn) { sten3(b.n, 0, b); return b.n; }
     return b.rows_ortho;
   }
   int from_ortho(const Base1& b) {
     if (b.cdn) { sten3(b.m, 1, b); pdma(b.m, b.d_pent.d, b.pent_L); return b.m; }
-    if (b.composite) {
-      band(b.m, b.n, 0, nullptr, 2, b.d_s2.d);
-      fdma(b.m, b.d_tfl.d, b.d_tid.d, b.d_tu1.d, nullptr, FD_NOU2);
-      return b.m;
-    }
+    if (b.composite) { band_solve(b.m, b.n, nullptr, b.bs2, nullptr, b.tlu); return b.m; }
     return b.rows_spec;
   }
   int deriv_axis(const Base1& b, int d, double sc) {  // on ortho coefficients; sc = 1/scale^d
@@ -734,10 +780,10 @@ struct Prog {
     o->i0 = b.rows_ortho;
     if (b.cdn) err = fail(B2_ERR_UNSUPPORTED, "stencil-on-load is pair-structured (ChebDirichletNeumann uses OP_STEN3)");
     o->i2 = (acc ? LD_ACC : 0) | (b.composite ? LD_STENCIL : 0);
-    o->p1 = b.d_sten2.d;
+    o->p1 = b.bsten.nat.d;
   }
   int matvec(const Base1& b) {          // MatVecFdma with pinv (Chebyshev axes only)
-    if (b.composite || b.cdn) { band(b.m, b.n, 0, b.d_bd.d, 2, b.d_bu1.d, 4, b.d_bu2.d); return b.m; }
+    if (b.composite || b.cdn) { band(b.m, b.n, &b.bd, 2, b.bu1, &b.bu2); return b.m; }
     return b.rows_spec;
   }
 };
@@ -756,10 +802,13 @@ template <int E, int LN, int TPLC> static int launch_ELT(b2_ctx* ctx, const Pass
 // Kernel instances: transform-sized lanes (c.fast) get the compile-time-geometry instance of their (E, LN, TPL);
 // every other geometry runs the generic instance of its (E, LN).
 static int launch_pass(b2_ctx* ctx, const PassCfg& c, const LaneProg& p) {
-#define B2_INST(e, ln, tpl) if (c.fast && c.E == e && c.LN == ln && c.TPL == tpl) return launch_ELT<e, ln, tpl>(ctx, c, p);
-  B2_INST(16, 4, 128) B2_INST(16, 4, 64) B2_INST(16, 4, 32) B2_INST(16, 4, 16) B2_INST(16, 4, 8)
-  B2_INST(16, 2, 256) B2_INST(16, 2, 128)
+// the (E, LN, TPL) combinations with a compile-time-geometry instance (also read by has_fast_instance)
+#define B2_FAST_INSTANCES \
+  B2_INST(16, 4, 128) B2_INST(16, 4, 64) B2_INST(16, 4, 32) B2_INST(16, 4, 16) B2_INST(16, 4, 8) \
+  B2_INST(16, 2, 256) B2_INST(16, 2, 128) \
   B2_INST(8, 4, 64) B2_INST(8, 4, 32) B2_INST(8, 4, 16) B2_INST(8, 4, 8) B2_INST(4, 4, 8) B2_INST(4, 4, 16) B2_INST(4, 4, 32)
+#define B2_INST(e, ln, tpl) if (c.fast && c.E == e && c.LN == ln && c.TPL == tpl) return launch_ELT<e, ln, tpl>(ctx, c, p);
+  B2_FAST_INSTANCES
 #undef B2_INST
   if (c.LN == 4) {
     if (c.E == 16) return launch_ELT<16, 4, 0>(ctx, c, p);
@@ -770,17 +819,24 @@ static int launch_pass(b2_ctx* ctx, const PassCfg& c, const LaneProg& p) {
   if (c.E == 8) return launch_ELT<8, 2, 0>(ctx, c, p);
   return launch_ELT<4, 2, 0>(ctx, c, p);
 }
+// Only lanes with a compile-time-geometry instance are transform-sized (PassCfg::fast) and get the fast op forms (OP_BANDC,
+// OP_PREBAND, chunk-map solves): the generic instances do not implement them.
+static bool has_fast_instance(int E, int LN, int TPL) {
+#define B2_INST(e, ln, tpl) if (E == e && LN == ln && TPL == tpl) return true;
+  B2_FAST_INSTANCES
+#undef B2_INST
+  return false;
+}
 
 static bool g_use_tma = getenv("B2_NOTMA") == nullptr;     // B2_NOTMA=1: every load/store on the per-thread LDG/STG path (A/B measurements)
 static bool g_use_ring = getenv("B2_LDTHREADS") == nullptr;  // combining loads (accumulate / multiply / stencil / scaled) stream through the warps' own
                                                              // copy pipelines (load_warps); B2_LDTHREADS=1: per-thread 16-byte loads instead
 
-// orient 0: lanes along axis 1; orient 1: lanes along axis 0
-static int run_pass(b2_space* sp, int orient, Prog& pr) {
+static int run_pass(Prog& pr) {
   if (pr.err != B2_OK) return pr.err;
-  const PassCfg& c = sp->cfg[orient];
+  const PassCfg& c = pr.c;
   LaneProg& p = pr.p;
-  b2_ctx* ctx = sp->ctx;
+  b2_ctx* ctx = pr.sp->ctx;
   p.LP = c.LP; p.in_tiles = c.in_tiles; p.out_tiles = c.out_tiles; p.TPL = c.TPL; p.C = c.C;
   p.group0 = ctx->rank * (c.groups / ctx->nranks); p.groups_per_rank = c.in_tiles / ctx->nranks; p.rank = ctx->rank;
   p.prof = ctx->d_prof; p.LN = c.LN;
@@ -795,73 +851,6 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
       else if (p.ops[i].code == OP_STORE && (p.ops[i].i2 & ST_COLSPLIT)) { p.ops[i].p1 = ctx->d_peers; exchange = true; }
   } else {
     for (int i = 0; i < p.nops; i++) if (p.ops[i].code == OP_STORE) p.ops[i].i2 &= ~ST_COLSPLIT;   // one GPU: a plain same-orientation store
-  }
-  // Generic geometry: a tiled load followed by the composite -> orthonormal stencil (to_ortho: y_j = x_j + s_j x_{j-2}) becomes
-  // ONE load that applies the stencil on the fly (LD_STENCIL).  Transform-sized lanes keep the zero-copy load and run the
-  // stencil as a chunk-streaming band op instead (on C4 stencil-on-load through the staging slots took longer per lane group
-  // than the zero-copy load and band_chunk together).
-  for (int i = 0; !c.fast && i + 1 < p.nops; i++) {
-    LaneOp& lo = p.ops[i]; LaneOp& bo = p.ops[i + 1];
-    if (lo.code != OP_LOAD || (lo.i2 & (LD_PLAIN | LD_STENCIL | LD_ACC | LD_MUL)) || bo.code != OP_BAND) continue;
-    const int h0 = (int)(signed char)(bo.i1 & 0xff), h1 = (int)(signed char)((bo.i1 >> 8) & 0xff), h2 = (int)(signed char)((bo.i1 >> 16) & 0xff);
-    if (h0 != 0 || bo.p0 != nullptr || h1 != -2 || bo.p1 == nullptr || h2 != 127 || bo.i2 != lo.i0) continue;   // not to_ortho of what was loaded
-    lo.i2 |= LD_STENCIL; lo.p1 = bo.p1; lo.i0 = bo.i0;
-    bo.code = OP_PREBAND;   // no-op
-  }
-  // Fold a banded mat-vec into the LU solve that consumes it (forward offsets only, same output length; shared
-  // coefficient vectors): the solve forms its right-hand side on the fly (lane_fast.cuh, fdma_fast_body<PREBAND>).
-  // Faster on C2 (E = 8), slower on C4 (E = 16, where the extra coefficient streams cost more than the saved
-  // pass; still 0.14 ms per step slower with the chunk-map solve, H100 SXM at 400 W), so it is applied to the short-lane
-  // instances only.
-  if (c.fast && c.E <= 8) {
-    for (int i = 0; i + 1 < p.nops; i++) {
-      LaneOp& bo = p.ops[i]; LaneOp& fo = p.ops[i + 1];
-      if (bo.code != OP_BAND || fo.code != OP_FDMA || (fo.i2 & FD_PERLANE) || bo.i0 != fo.i0) continue;
-      bool ok = true;
-      const void* sc[3] = {nullptr, nullptr, nullptr};
-      const void* nat[3] = {bo.p0, bo.p1, bo.p2};
-      for (int m = 0; m < 3; m++) {
-        const int h = (int)(signed char)((bo.i1 >> (8 * m)) & 0xff);
-        if (h == 127) continue;
-        if (h != 0 && h != 2 && h != 4) ok = false;
-        if (nat[m]) { auto it = scan_of().find(nat[m]); if (it == scan_of().end()) ok = false; else sc[m] = it->second; }
-      }
-      if (!ok) continue;
-      bo.code = OP_PREBAND; bo.p0 = sc[0]; bo.p1 = sc[1]; bo.p2 = sc[2]; fo.i2 |= FD_PREBAND;
-    }
-  }
-  // LU solves with shared coefficient vectors run on their chunk-map table on transform-sized lanes (fdma_fast_body)
-  for (int i = 0; c.fast && i < p.nops; i++) {
-    LaneOp& fo = p.ops[i];
-    if (fo.code != OP_FDMA || (fo.i2 & FD_PERLANE)) continue;
-    const auto it = lumap_of().find(fo.p0);
-    if (it == lumap_of().end() || it->second.C != c.C || it->second.TPL != c.TPL)
-      return fail(B2_ERR_ARG, "LU solve without a chunk-map table for this lane layout");
-    fo.p0 = it->second.table;
-  }
-  // Remaining banded mat-vecs on transform-sized lanes run in chunk-streaming form (band_chunk: one read and one write
-  // traversal of the lane group): pair offsets {0, +1, +2} or {0, -1}, vector coefficients through their scan-layout copies.
-  if (c.fast) {
-    for (int i = 0; i < p.nops; i++) {
-      LaneOp& bo = p.ops[i];
-      if (bo.code != OP_BAND) continue;
-      const void* nat[3] = {bo.p0, bo.p1, bo.p2};
-      const void* slot[3] = {nullptr, nullptr, nullptr};
-      int flag[3] = {0, 0, 0};
-      bool ok = true, anyvec = false, fwd = false, bwd = false;
-      for (int m = 0; m < 3 && ok; m++) {
-        const int h = (int)(signed char)((bo.i1 >> (8 * m)) & 0xff);
-        if (h == 127) continue;
-        int k;
-        if (h == 0) k = 0; else if (h == 2) { k = 1; fwd = true; } else if (h == 4) { k = 2; fwd = true; } else if (h == -2) { k = 1; bwd = true; } else { ok = false; break; }
-        if (flag[k]) { ok = false; break; }
-        if (nat[m]) { auto it = scan_of().find(nat[m]); if (it == scan_of().end()) { ok = false; break; } slot[k] = it->second; flag[k] = 2; anyvec = true; }
-        else flag[k] = 1;
-      }
-      if (!ok || !anyvec || (fwd && bwd)) continue;
-      bo.code = OP_BANDC; bo.p0 = slot[0]; bo.p1 = slot[1]; bo.p2 = slot[2];
-      bo.i1 = (bwd ? 1 : 0) | (flag[0] << 2) | (flag[1] << 4) | (flag[2] << 6);
-    }
   }
   // TMA views.  Arrays are 4x4-tiled: tile (I, J) at ((I * tiles_per_row) + J) * 128 bytes, element [i][j] inside.
   //   slab view (loads, same-orientation stores): [16 doubles of a tile][tile J of the lane group][lane group]
@@ -948,7 +937,7 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
     if (e != cudaSuccess) {
       std::string ops;
       for (int i = 0; i < p.nops; i++) ops += std::to_string(p.ops[i].code) + ":" + std::to_string(p.ops[i].i2) + " ";
-      return fail(B2_ERR_CUDA, std::string("pass failed (") + cudaGetErrorString(e) + "), orient " + std::to_string(orient) + ", ops code:flags = " + ops);
+      return fail(B2_ERR_CUDA, std::string("pass failed (") + cudaGetErrorString(e) + "), orient " + std::to_string(pr.orient) + ", ops code:flags = " + ops);
     }
   }
   return exchange ? ctx_barrier(ctx) : B2_OK;
@@ -957,15 +946,6 @@ static int run_pass(b2_space* sp, int orient, Prog& pr) {
 // ------------------------------------------------------------------------------------------------
 // context / space / arrays
 // ------------------------------------------------------------------------------------------------
-// the (E, LN, TPL) combinations that have a compile-time-geometry kernel instance (launch_pass): only those may run the
-// launcher's fast-geometry rewrites (OP_BANDC, OP_PREBAND) -- the generic instances do not implement them
-static bool has_fast_instance(int E, int LN, int TPL) {
-  if (LN == 2) return E == 16 && (TPL == 256 || TPL == 128);
-  if (E == 16) return TPL == 128 || TPL == 64 || TPL == 32 || TPL == 16 || TPL == 8;
-  if (E == 8) return TPL == 64 || TPL == 32 || TPL == 16 || TPL == 8;
-  if (E == 4) return TPL == 8 || TPL == 16 || TPL == 32;
-  return false;
-}
 static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nranks) {
   c->in_tiles = Pl / 4; c->out_tiles = Pc / 4; c->groups = Pc / 4; c->LP = Pl;
   const int N = lane_base.N;
@@ -1075,50 +1055,50 @@ static bool shape_complex(const b2_space* sp, int shape_kind) { return !sp->b[0]
 static int op_forward(b2_space* sp, const double* v, double* vhat) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64 runs the FFT core, other sizes up to 2049 a dense matrix; larger non-power-of-two sizes are not supported");
-  Prog y; y.load(v, b1.rows_phys); y.forward_ortho(b1); int l = y.from_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_phys); x.forward_ortho(b0); l = x.from_ortho(b0); x.store(vhat, l, ST_TRANS);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(v, b1.rows_phys); y.forward_ortho(b1); int l = y.from_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_phys); x.forward_ortho(b0); l = x.from_ortho(b0); x.store(vhat, l, ST_TRANS);
+  return run_pass(x);
 }
 static int op_backward(b2_space* sp, const double* vhat, double* v) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64 runs the FFT core, other sizes up to 2049 a dense matrix; larger non-power-of-two sizes are not supported");
-  Prog y; y.load(vhat, b1.rows_spec); y.to_ortho(b1); int l = y.backward_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_spec); x.to_ortho(b0); l = x.backward_ortho(b0); x.store(v, l, ST_TRANS);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(vhat, b1.rows_spec); y.to_ortho(b1); int l = y.backward_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); x.to_ortho(b0); l = x.backward_ortho(b0); x.store(v, l, ST_TRANS);
+  return run_pass(x);
 }
 static int op_to_ortho(b2_space* sp, const double* vhat, double* out, double alpha = 1.0, bool acc = false) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
-  Prog y; y.load(vhat, b1.rows_spec); int l = y.to_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_spec); l = x.to_ortho(b0); x.store(out, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(vhat, b1.rows_spec); int l = y.to_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); l = x.to_ortho(b0); x.store(out, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
+  return run_pass(x);
 }
 static int op_from_ortho(b2_space* sp, const double* in, double* vhat, double alpha = 1.0, bool acc = false) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
-  Prog y; y.load(in, b1.rows_ortho); int l = y.from_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_ortho); l = x.from_ortho(b0); x.store(vhat, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(in, b1.rows_ortho); int l = y.from_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_ortho); l = x.from_ortho(b0); x.store(vhat, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
+  return run_pass(x);
 }
 static int op_gradient(b2_space* sp, const double* vhat, int d0, int d1, const double* scale, double* out, double alpha = 1.0, bool acc = false) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   double s0 = 1.0, s1 = 1.0;
   if (scale) { s0 = 1.0 / std::pow(scale[0], d0); s1 = 1.0 / std::pow(scale[1], d1); }
-  Prog y; y.load(vhat, b1.rows_spec); y.to_ortho(b1); int l = y.deriv_axis(b1, d1, s1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_spec); x.to_ortho(b0); l = x.deriv_axis(b0, d0, s0); x.store(out, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(vhat, b1.rows_spec); y.to_ortho(b1); int l = y.deriv_axis(b1, d1, s1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); x.to_ortho(b0); l = x.deriv_axis(b0, d0, s0); x.store(out, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
+  return run_pass(x);
 }
 // transforms of an orthonormal ("field" = ch x ch or r2c x ch) array, funspace backward_par / forward
 static int op_backward_ortho(b2_space* sp, const double* ortho, double* phys) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size");
-  Prog y; y.load(ortho, b1.rows_ortho); int l = y.backward_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_ortho); l = x.backward_ortho(b0); x.store(phys, l, ST_TRANS);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(ortho, b1.rows_ortho); int l = y.backward_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_ortho); l = x.backward_ortho(b0); x.store(phys, l, ST_TRANS);
+  return run_pass(x);
 }
 // forward + dealias (src/navier_stokes/functions.rs:72-82), result scaled by alpha
 static int op_forward_ortho_dealias(b2_space* sp, const double* phys, double* ortho, bool dealias, double alpha = 1.0, bool acc = false) {
@@ -1127,22 +1107,16 @@ static int op_forward_ortho_dealias(b2_space* sp, const double* phys, double* or
   // bit-exact index rule: n_x = shape0*2/3, n_y = shape1*2/3 with integer division on the spectral shape
   const int shape0 = b0.cheb ? b0.n : b0.m, shape1 = b1.cheb ? b1.n : b1.m;
   const int cut0 = (shape0 * 2 / 3) * (b0.cheb ? 1 : 2), cut1 = (shape1 * 2 / 3) * (b1.cheb ? 1 : 2);
-  Prog y; y.load(phys, b1.rows_phys); int l = y.forward_ortho(b1); if (dealias) y.zerotail(cut1); y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_phys); l = x.forward_ortho(b0); if (dealias) x.zerotail(cut0);
+  Prog y(sp, 0); y.load(phys, b1.rows_phys); int l = y.forward_ortho(b1); if (dealias) y.zerotail(cut1); y.store(sp->tmp[0], l, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_phys); l = x.forward_ortho(b0); if (dealias) x.zerotail(cut0);
   x.store(ortho, l, ST_TRANS | (acc ? ST_ACC : 0), alpha);
-  return run_pass(sp, 1, x);
+  return run_pass(x);
 }
 
 // ------------------------------------------------------------------------------------------------
 // solvers
 // ------------------------------------------------------------------------------------------------
-static int upload_lu(const LuVecs& lu, const Base1& b, DVecD* fl, DVecD* id, DVecD* u1, DVecD* u2, DVecD* map) {
-  const std::vector<double> sfl = b.scan_layout(lu.fl), sid = b.scan_layout(lu.id), su1 = b.scan_layout(lu.u1), su2 = b.scan_layout(lu.u2);
-  RET(fl->upload(sfl)); RET(id->upload(sid)); RET(u1->upload(su1)); RET(u2->upload(su2));
-  return upload_lu_maps(fl->d, sfl, sid, su1, &su2, b.lay_C, b.lay_TPL, map);
-}
-
 static int hholtz_create(b2_space* sp, double c0, double c1, b2_solver** out) {
   b2_solver* s = new b2_solver();
   s->sp = sp; s->type = 0;
@@ -1158,7 +1132,7 @@ static int hholtz_create(b2_space* sp, double c0, double c1, b2_solver** out) {
         mat.up1[i] = a.up1[i] - bm.up1[i] * c[ax];
         mat.up2[i] = a.up2[i] - bm.up2[i] * c[ax];
       }
-      RET(upload_lu(sweep(mat), b, &s->fl[ax], &s->id[ax], &s->u1[ax], &s->u2[ax], &s->lm[ax]));
+      RET(upload_lu(sweep(mat), true, b.lay_C, b.lay_TPL, &s->lu[ax]));
     } else if (b.cdn) {  // PdmaPlus2::from_matrix(mat), src/solver/hholtz_adi.rs:64
       std::vector<double> d[7];
       b.cdn_hholtz_diags(c[ax], d);
@@ -1185,12 +1159,12 @@ static void emit_hh_axis(Prog& p, const b2_solver* s, int ax);
 static int hholtz_solve(b2_solver* s, const double* in, double* out) {
   b2_space* sp = s->sp;
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
-  Prog y; y.load(in, b1.rows_ortho); emit_hh_axis(y, s, 1);
+  Prog y(sp, 0); y.load(in, b1.rows_ortho); emit_hh_axis(y, s, 1);
   y.store(sp->tmp[0], b1.rows_spec, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_ortho); emit_hh_axis(x, s, 0);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_ortho); emit_hh_axis(x, s, 0);
   x.store(out, b0.rows_spec, ST_TRANS);
-  return run_pass(sp, 1, x);
+  return run_pass(x);
 }
 
 // laplacian / mass of axis ax as in Poisson::new (src/solver/poisson.rs:65-74)
@@ -1310,7 +1284,7 @@ static int poisson_create(b2_space* sp, double c0, double c1, const double* lam_
   const int nr = sp->ctx->nranks, lane0 = sp->ctx->rank * (c.groups / nr) * 4, lane1 = lane0 + (c.groups / nr) * 4;
   const size_t total = (size_t)(c.groups / nr) * c.C * 4 * c.TPL * 2;
   const int m1 = b1.m;
-  auto build_lanes = [&](const std::vector<double>& lamv, DVecD* dfl, DVecD* did, DVecD* du1, DVecD* du2) -> int {
+  auto build_lanes = [&](const std::vector<double>& lamv, LuDev* d) -> int {
     std::vector<double> pfl(total, 0.0), pid(total, 0.0), pu1(total, 0.0), pu2(total, 0.0);
     Diags mat(m1);
     for (int lane = lane0; lane < std::min(lanes, lane1); lane++) {
@@ -1329,10 +1303,11 @@ static int poisson_create(b2_space* sp, double c0, double c1, const double* lam_
         pfl[k] = lu.fl[i]; pid[k] = lu.id[i]; pu1[k] = lu.u1[i]; pu2[k] = lu.u2[i];
       }
     }
-    RET(dfl->upload(pfl)); RET(did->upload(pid)); RET(du1->upload(pu1)); RET(du2->upload(pu2));
+    d->C = c.C; d->TPL = c.TPL; d->perlane = true;
+    RET(d->fl.upload(pfl)); RET(d->id.upload(pid)); RET(d->u1.upload(pu1)); RET(d->u2.upload(pu2));
     return B2_OK;
   };
-  RET(build_lanes(lam, &s->pfl, &s->pid, &s->pu1, &s->pu2));
+  RET(build_lanes(lam, &s->pl));
   if (s->dense) {
     // parity classes of the modes: row r of fwd (= mode r) touches even columns only, or odd columns only
     const int m0 = s->m0, ce = (m0 + 1) / 2, co = m0 / 2;
@@ -1354,7 +1329,7 @@ static int poisson_create(b2_space* sp, double c0, double c1, const double* lam_
       for (int r = 0; r < ce; r++) for (int k = 0; k < ce; k++) { fe[(size_t)r * ce + k] = fwd[(size_t)perm[r] * m0 + 2 * k]; be[(size_t)k * ce + r] = bwd[(size_t)(2 * k) * m0 + perm[r]]; }
       for (int r = 0; r < co; r++) for (int k = 0; k < co; k++) { fo[(size_t)r * co + k] = fwd[(size_t)perm[ce + r] * m0 + 2 * k + 1]; bo[(size_t)k * co + r] = bwd[(size_t)(2 * k + 1) * m0 + perm[ce + r]]; }
       for (int r = 0; r < m0; r++) lam2[r] = lam[perm[r]];
-      RET(build_lanes(lam2, &s->qfl, &s->qid, &s->qu1, &s->qu2));
+      RET(build_lanes(lam2, &s->ql));
       s->blocks = true; s->ce = ce; s->co = co;
       RET(gemm_plan_create(sp, &s->gf, fe.data(), ce, ce, fo.data(), co, co, true, false));   // forward: natural x rows -> modes grouped by class
       RET(gemm_plan_create(sp, &s->gb, be.data(), ce, ce, bo.data(), co, co, false, true));   // backward: the reverse
@@ -1387,18 +1362,17 @@ static int gemm_mark(b2_ctx* ctx) {
 static int poisson_core(b2_solver* s, b2_space* rs, const double* src, bool matvec_y, double* gx, double* y1, double* out, bool zero00) {
   b2_ctx* ctx = rs->ctx;
   const Base1& b1 = s->sp->b[1];
-  Prog y; y.load(src, matvec_y ? b1.rows_ortho : b1.m);
+  Prog y(rs, 0); y.load(src, matvec_y ? b1.rows_ortho : b1.m);
   if (matvec_y) y.matvec(b1);
   y.store(gx, b1.m, ST_COLSPLIT);
-  RET(run_pass(rs, 0, y));
+  RET(run_pass(y));
   RET(gemm_mark(ctx));
   RET(gemm_run(ctx, s->gf, gx, y1));   // forward: x index -> eigenmodes (parity blocks: modes grouped by class, the order of q*)
   RET(gemm_mark(ctx));
-  Prog y2; y2.load(y1, b1.m);
-  if (s->blocks) y2.fdma(b1.m, s->qfl.d, s->qid.d, s->qu1.d, s->qu2.d, FD_PERLANE);
-  else y2.fdma(b1.m, s->pfl.d, s->pid.d, s->pu1.d, s->pu2.d, FD_PERLANE);
+  Prog y2(rs, 0); y2.load(y1, b1.m);
+  y2.fdma(b1.m, s->blocks ? s->ql : s->pl);
   y2.store(gx, b1.m, ST_COLSPLIT);
-  RET(run_pass(rs, 0, y2));
+  RET(run_pass(y2));
   RET(gemm_mark(ctx));
   RET(gemm_run(ctx, s->gb, gx, out));  // backward: eigenmodes -> x index (natural order)
   RET(gemm_mark(ctx));
@@ -1414,28 +1388,28 @@ static int poisson_solve(b2_solver* s, const double* in, double* out, bool zero0
   const int P0 = sp->P[0], P1 = sp->P[1];
   if (s->dense) {
     // matvec along y and x (two transposing passes: back in the y-lane orientation, rows = x index), then the core
-    Prog y; y.load(in, b1.rows_ortho); int l = y.matvec(b1); y.store(sp->tmp[0], l, ST_TRANS);
-    RET(run_pass(sp, 0, y));
-    Prog x; x.load(sp->tmp[0], b0.rows_ortho); l = x.matvec(b0); x.store(sp->tmp[1], l, ST_TRANS);
-    RET(run_pass(sp, 1, x));
+    Prog y(sp, 0); y.load(in, b1.rows_ortho); int l = y.matvec(b1); y.store(sp->tmp[0], l, ST_TRANS);
+    RET(run_pass(y));
+    Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_ortho); l = x.matvec(b0); x.store(sp->tmp[1], l, ST_TRANS);
+    RET(run_pass(x));
     return poisson_core(s, sp, sp->tmp[1], false, sp->tmp[0], sp->tmp[2], out, zero00);
   }
-  Prog y; y.load(in, b1.rows_ortho); int l = y.matvec(b1);
-  y.fdma(b1.m, s->pfl.d, s->pid.d, s->pu1.d, s->pu2.d, FD_PERLANE);
+  Prog y(sp, 0); y.load(in, b1.rows_ortho); int l = y.matvec(b1);
+  y.fdma(b1.m, s->pl);
   y.store(sp->tmp[0], l, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_spec);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec);
   if (zero00) { x.zeroelem(0, 0); x.zeroelem(0, 1); }
   x.store(out, b0.rows_spec, ST_TRANS);
-  return run_pass(sp, 1, x);
+  return run_pass(x);
 }
 
 // one axis of HholtzAdi: precondition (MatVecFdma) + banded / diagonal solve
 static void emit_hh_axis(Prog& p, const b2_solver* s, int ax) {
   const Base1& b = s->sp->b[ax];
+  if (b.composite) { p.band_solve(b.m, b.n, &b.bd, b.bu1, &b.bu2, s->lu[ax]); return; }
   p.matvec(b);
-  if (b.composite) p.fdma(b.m, s->fl[ax].d, s->id[ax].d, s->u1[ax].d, s->u2[ax].d, 0);
-  else if (b.cdn) p.pdma(b.m, s->pd[ax].d, s->pd_L[ax]);   // hholtz_adi.rs:64
+  if (b.cdn) p.pdma(b.m, s->pd[ax].d, s->pd_L[ax]);   // hholtz_adi.rs:64
   else p.scalevec(b.rows_spec, s->sd[ax].d, 1);
 }
 
@@ -1574,10 +1548,10 @@ int b2_debug_copy(b2_space* sp, int mode, int reps, double* ms) {
   b2_ctx* ctx = sp->ctx;
   const Base1& by = sp->b[1];
   auto pass = [&]() -> int {
-    Prog y; y.load(a, by.rows_ortho, (mode & 4) ? 2.0 : 1.0);
+    Prog y(sp, 0); y.load(a, by.rows_ortho, (mode & 4) ? 2.0 : 1.0);
     if (mode & 2) y.dct(by, 1);
     y.store(b, by.rows_ortho, (mode & 1) ? ST_TRANS : 0, (mode & 8) ? 2.0 : 1.0);
-    return run_pass(sp, 0, y);
+    return run_pass(y);
   };
   RET(pass());
   if (!ctx->ev0) { CK(cudaEventCreate(&ctx->ev0)); CK(cudaEventCreate(&ctx->ev1)); }
@@ -1860,10 +1834,10 @@ int b2_field_dealias(b2_field* f) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   if (b0.c2c) return fail(B2_ERR_UNSUPPORTED, "dealias: the 2/3 tail rule of functions.rs:72-82 is written for r2c / Chebyshev mode order");
   const int cut0 = (b0.m * 2 / 3) * (b0.cheb ? 1 : 2), cut1 = b1.m * 2 / 3;
-  Prog y; y.load(f->vhat->d, b1.rows_spec); y.zerotail(cut1); y.store(sp->tmp[0], b1.rows_spec, ST_TRANS);
-  RET(run_pass(sp, 0, y));
-  Prog x; x.load(sp->tmp[0], b0.rows_spec); x.zerotail(cut0); x.store(f->vhat->d, b0.rows_spec, ST_TRANS);
-  return run_pass(sp, 1, x);
+  Prog y(sp, 0); y.load(f->vhat->d, b1.rows_spec); y.zerotail(cut1); y.store(sp->tmp[0], b1.rows_spec, ST_TRANS);
+  RET(run_pass(y));
+  Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); x.zerotail(cut0); x.store(f->vhat->d, b0.rows_spec, ST_TRANS);
+  return run_pass(x);
 }
 
 int b2_hholtz_adi_create(const b2_field* f, double c0, double c1, b2_solver** out) { return hholtz_create(f->sp, c0, c1, out); }
@@ -1876,11 +1850,9 @@ int b2_hholtz_create(const b2_field* f, double c0, double c1, const double* lam,
 int b2_solver_destroy(b2_solver* s) {
   if (!s) return B2_OK;
   for (int ax = 0; ax < 2; ax++) {
-    if (s->fl[ax].d) lumap_of().erase(s->fl[ax].d);
-    s->fl[ax].release(); s->id[ax].release(); s->u1[ax].release(); s->u2[ax].release(); s->sd[ax].release(); s->pd[ax].release(); s->lm[ax].release();
+    s->lu[ax].release(); s->sd[ax].release(); s->pd[ax].release();
   }
-  s->pfl.release(); s->pid.release(); s->pu1.release(); s->pu2.release();
-  s->qfl.release(); s->qid.release(); s->qu1.release(); s->qu2.release();
+  s->pl.release(); s->ql.release();
   for (GemmPlan* g : {&s->gf, &s->gb}) { g->A[0].release(); g->A[1].release(); }
   delete s;
   return B2_OK;
@@ -1989,16 +1961,16 @@ int b2_navier2d_create(b2_ctx* ctx, int nx, int ny, double ra, double pr, double
     // GxT / GyT = backward(d/dx tempbc), backward(d/dy tempbc): physical values, kept in x-lane orientation
     for (int d = 0; d < 2; d++) {
       RET(op_gradient(so, nv->tempbc->vhat->d, d == 0, d == 1, nv->scale, nv->g1));
-      Prog y; y.load(nv->g1, byo.rows_ortho); int l = y.backward_ortho(byo); y.store(so->tmp[0], l, ST_TRANS);
-      RET(run_pass(so, 0, y));
-      Prog x; x.load(so->tmp[0], bxo.rows_ortho); l = x.backward_ortho(bxo); x.store(d == 0 ? nv->GxT : nv->GyT, l, 0);
-      RET(run_pass(so, 1, x));
+      Prog y(so, 0); y.load(nv->g1, byo.rows_ortho); int l = y.backward_ortho(byo); y.store(so->tmp[0], l, ST_TRANS);
+      RET(run_pass(y));
+      Prog x(so, 1); x.load(so->tmp[0], bxo.rows_ortho); l = x.backward_ortho(bxo); x.store(d == 0 ? nv->GxT : nv->GyT, l, 0);
+      RET(run_pass(x));
     }
     // KbT = dt * Hholtz_vely(to_ortho(tempbc)); KTT = Hholtz_temp(dt ka lap tempbc); both transposed
     RET(hholtz_solve(nv->hh[1], nv->tbc_ortho, nv->g1));
-    { Prog y; y.load(nv->g1, so->P[1], dt); y.store(nv->KbT, so->P[1], ST_TRANS); RET(run_pass(so, 0, y)); }
+    { Prog y(so, 0); y.load(nv->g1, so->P[1], dt); y.store(nv->KbT, so->P[1], ST_TRANS); RET(run_pass(y)); }
     RET(hholtz_solve(nv->hh[2], nv->tbc_diff, nv->g1));
-    { Prog y; y.load(nv->g1, so->P[1]); y.store(nv->KTT, so->P[1], ST_TRANS); RET(run_pass(so, 0, y)); }
+    { Prog y(so, 0); y.load(nv->g1, so->P[1]); y.store(nv->KTT, so->P[1], ST_TRANS); RET(run_pass(y)); }
   }
   CK(cudaStreamSynchronize(ctx->stream));
   *out = nv;
@@ -2141,11 +2113,11 @@ static int nav_update_fused(b2_navier* nv) {
   RET(after(1, 0)); RET(after(2, 0));   // fork
   {  // branch 2 first: pressure gradient terms, Helmholtz-y of pres and of d/dy pres
     on(2);
-    Prog y;
+    Prog y(so, 0);
     // (the factor -dt of the pressure-gradient terms rides on the transposing stores: the consumers' loads stay zero-copy)
     y.load(nv->pres->vhat->d, byo.rows_ortho); emit_hh_axis(y, nv->hh[0], 1); y.store(nv->PH, nv->sp_vel->b[1].m, ST_TRANS, -dt);
     y.load(nv->pres->vhat->d, byo.rows_ortho); y.deriv_axis(byo, 1, sy); emit_hh_axis(y, nv->hh[1], 1); y.store(nv->PHy, nv->sp_vel->b[1].m, ST_TRANS, -dt);
-    RET(run_pass(so, 0, y));
+    RET(run_pass(y));
   }
   // ---- A: along y on the three advected fields: values, d/dy values, Helmholtz-y of the old field ----
   for (int i = 0; i < 3; i++) {
@@ -2153,7 +2125,7 @@ static int nav_update_fused(b2_navier* nv) {
     const b2_field* f = fld[i];
     const Base1& by = f->sp->b[1];
     const double* src = f->vhat->d;
-    Prog y;
+    Prog y(so, 0);
     // the orthonormal image of the lanes is needed three (four) times: project once, keep a copy (a zero-copy slab store and
     // zero-copy reloads) instead of repeating the stencil pass after every reload of the composite coefficients
     y.load(src, by.rows_spec); int lo = y.to_ortho(by); y.store(nv->Of[i], lo, 0);
@@ -2161,21 +2133,21 @@ static int nav_update_fused(b2_navier* nv) {
     y.load(nv->Of[i], lo); y.deriv_axis(by, 1, sy); l = y.backward_ortho(by); y.store(nv->Qf[i], l, ST_TRANS);
     y.load(nv->Of[i], lo); emit_hh_axis(y, nv->hh[i], 1); y.store(nv->V1[i], by.m, ST_TRANS);
     if (i == 2) { y.load(nv->Of[i], lo); emit_hh_axis(y, nv->hh[1], 1); y.store(nv->VTv, by.m, ST_TRANS); }
-    RET(run_pass(so, 0, y));
+    RET(run_pass(y));
   }
   // ---- A-x: convection velocities ux, uy (physical, x-lane orientation) ----
   for (int i = 0; i < 2; i++) {
     on(i);
     const Base1& bx = fld[i]->sp->b[0];
-    Prog x; x.load(nv->Pf[i], bx.rows_spec); x.to_ortho(bx); int l = x.backward_ortho(bx); x.store(i == 0 ? nv->uxT : nv->uyT, l, 0);
-    RET(run_pass(so, 1, x));
+    Prog x(so, 1); x.load(nv->Pf[i], bx.rows_spec); x.to_ortho(bx); int l = x.backward_ortho(bx); x.store(i == 0 ? nv->uxT : nv->uyT, l, 0);
+    RET(run_pass(x));
   }
   RET(after(1, 0)); RET(after(0, 1)); RET(after(2, 0)); RET(after(2, 1));   // every branch needs ux and uy
   // ---- B: u . grad f in physical space, forward transform along x, dealias rows ----
   for (int i = 0; i < 3; i++) {
     on(i);
     const Base1& bx = fld[i]->sp->b[0];
-    Prog x;
+    Prog x(so, 1);
     x.load(nv->Pf[i], bx.rows_spec); x.to_ortho(bx); x.deriv_axis(bx, 1, sx); int l = x.backward_ortho(bx);
     if (i == 2) x.load(nv->GxT, l, 1.0, LD_ACC);
     x.load(nv->uxT, l, 1.0, LD_MUL);
@@ -2186,29 +2158,29 @@ static int nav_update_fused(b2_navier* nv) {
     x.load(nv->cv[i], l, 1.0, LD_ACC);
     l = x.forward_ortho(bxo); x.zerotail(cut0);
     x.store(nv->Cx[i], l, ST_TRANS, -dt);   // rhs -= dt * conv: the factor rides on the store
-    RET(run_pass(so, 1, x));
+    RET(run_pass(x));
   }
   // ---- C-y: forward along y, dealias columns, -dt, Helmholtz-y ----
   for (int i = 0; i < 3; i++) {
     on(i);
-    Prog y; y.load(nv->Cx[i], byo.rows_phys); y.forward_ortho(byo); y.zerotail(cut1);
+    Prog y(so, 0); y.load(nv->Cx[i], byo.rows_phys); y.forward_ortho(byo); y.zerotail(cut1);
     emit_hh_axis(y, nv->hh[i], 1); y.store(nv->Zf[i], fld[i]->sp->b[1].m, ST_TRANS);
-    RET(run_pass(so, 0, y));
+    RET(run_pass(y));
   }
   // ---- C-x: assemble rhs along x and finish the three Helmholtz solves ----
   RET(after(0, 2)); RET(after(1, 2));   // PH, PHy, VTv come from branch 2
   {
     const Base1& bxv = nv->sp_vel->b[0]; const Base1& bxT = nv->sp_temp->b[0];
     on(0);
-    Prog x;  // velx
+    Prog x(so, 1);  // velx
     x.load(nv->PH, bxo.rows_ortho); x.deriv_axis(bxo, 1, sx);
     x.load(nv->Zf[0], bxo.rows_ortho, 1.0, LD_ACC);
     x.load_stencil(nv->V1[0], bxv, 1.0, true);
     emit_hh_axis(x, nv->hh[0], 0);
     x.store(nv->velx->vhat->d, bxv.rows_spec, ST_TRANS);
-    RET(run_pass(so, 1, x));
+    RET(run_pass(x));
     on(1);
-    Prog v;  // vely (+ buoyancy dt * (to_ortho(temp) + to_ortho(tempbc)))
+    Prog v(so, 1);  // vely (+ buoyancy dt * (to_ortho(temp) + to_ortho(tempbc)))
     v.load(nv->PHy, bxo.rows_ortho);
     v.load(nv->Zf[1], bxo.rows_ortho, 1.0, LD_ACC);
     v.load_stencil(nv->V1[1], bxv, 1.0, true);
@@ -2216,36 +2188,36 @@ static int nav_update_fused(b2_navier* nv) {
     emit_hh_axis(v, nv->hh[1], 0);
     v.load(nv->KbT, bxv.rows_spec, 1.0, LD_ACC);
     v.store(nv->vely->vhat->d, bxv.rows_spec, ST_TRANS);
-    RET(run_pass(so, 1, v));
+    RET(run_pass(v));
   }
   // temperature Helmholtz (branch 2: it only needs the old fields and its own convection term)
   {
     on(2);
     const Base1& bxT = nv->sp_temp->b[0];
-    Prog t;
+    Prog t(so, 1);
     t.load(nv->Zf[2], bxo.rows_ortho);
     t.load_stencil(nv->V1[2], bxT, 1.0, true);
     emit_hh_axis(t, nv->hh[2], 0);
     t.load(nv->KTT, bxT.rows_spec, 1.0, LD_ACC);
     t.store(nv->temp->vhat->d, bxT.rows_spec, ST_TRANS);
-    RET(run_pass(so, 1, t));
+    RET(run_pass(t));
   }
   RET(after(0, 1));
   on(0);
   // ---- D: divergence of the intermediate velocity, pressure update part 1, Poisson rhs ----
   {
     const Base1& byv = nv->sp_vel->b[1]; const Base1& bxv = nv->sp_vel->b[0];
-    Prog y;
+    Prog y(so, 0);
     y.load(nv->velx->vhat->d, byv.rows_spec); int l = y.to_ortho(byv); y.store(nv->F1, l, ST_TRANS);
     y.load(nv->vely->vhat->d, byv.rows_spec); y.to_ortho(byv); l = y.deriv_axis(byv, 1, sy); y.store(nv->F2, l, ST_TRANS);
-    RET(run_pass(so, 0, y));
-    Prog x;
+    RET(run_pass(y));
+    Prog x(so, 1);
     x.load(nv->F1, bxv.rows_spec); x.to_ortho(bxv); x.deriv_axis(bxv, 1, sx);
     x.load_stencil(nv->F2, bxv, 1.0, true);
     x.store(nv->pres->vhat->d, bxo.rows_ortho, ST_TRANS | ST_ACC, -nv->nu);   // pres += -nu div (navier_eq.rs:137-143)
     x.matvec(bxp);
     x.store(nv->R0, bxp.rows_spec, ST_TRANS);
-    RET(run_pass(so, 1, x));
+    RET(run_pass(x));
   }
   // ---- Poisson (src/solver/poisson.rs:195-236) ----
   b2_solver* ps = nv->pois;
@@ -2254,16 +2226,16 @@ static int nav_update_fused(b2_navier* nv) {
     // around them is a zero-copy slab copy; with several GPUs the exchanges ride on those stores and on the GEMM epilogue
     RET(poisson_core(ps, so, nv->R0, true, nv->G0, nv->G1, nv->pseu->vhat->d, true));
   } else {
-    Prog y; y.load(nv->R0, byo.rows_ortho); y.matvec(byp);
-    y.fdma(byp.m, ps->pfl.d, ps->pid.d, ps->pu1.d, ps->pu2.d, FD_PERLANE);
+    Prog y(so, 0); y.load(nv->R0, byo.rows_ortho); y.matvec(byp);
+    y.fdma(byp.m, ps->pl);
     y.zeroelem(0, 0); y.zeroelem(1, 0);
     y.store(nv->pseu->vhat->d, byp.m, 0);
-    RET(run_pass(so, 0, y));
+    RET(run_pass(y));
   }
   // ---- E: velocity correction and pressure update part 2 (navier_eq.rs:117-143) ----
   {
     const Base1& byv = nv->sp_vel->b[1]; const Base1& bxv = nv->sp_vel->b[0];
-    Prog y;
+    Prog y(so, 0);
     for (int k = 0; k < 3; k++) {
       if (k == 0) { y.load(nv->pseu->vhat->d, byp.m); const int lo = y.to_ortho(byp); y.store(nv->G0, lo, 0); }   // (G0 is free again: one projection, two zero-copy reloads)
       else y.load(nv->G0, byo.rows_ortho);
@@ -2272,20 +2244,20 @@ static int nav_update_fused(b2_navier* nv) {
       if (k < 2) l = y.from_ortho(byv);
       y.store(k == 0 ? nv->U1 : (k == 1 ? nv->U2 : nv->U3), l, ST_TRANS);
     }
-    RET(run_pass(so, 0, y));
+    RET(run_pass(y));
     RET(after(1, 0)); RET(after(2, 0));
     on(0);
-    Prog x1; x1.load(nv->U1, bxp.rows_spec); x1.to_ortho(bxp); x1.deriv_axis(bxo, 1, sx); int l = x1.from_ortho(bxv);
+    Prog x1(so, 1); x1.load(nv->U1, bxp.rows_spec); x1.to_ortho(bxp); x1.deriv_axis(bxo, 1, sx); int l = x1.from_ortho(bxv);
     x1.store(nv->velx->vhat->d, l, ST_TRANS | ST_ACC, -1.0);
-    RET(run_pass(so, 1, x1));
+    RET(run_pass(x1));
     on(1);
-    Prog x2; x2.load(nv->U2, bxp.rows_spec); x2.to_ortho(bxp); l = x2.from_ortho(bxv);
+    Prog x2(so, 1); x2.load(nv->U2, bxp.rows_spec); x2.to_ortho(bxp); l = x2.from_ortho(bxv);
     x2.store(nv->vely->vhat->d, l, ST_TRANS | ST_ACC, -1.0);
-    RET(run_pass(so, 1, x2));
+    RET(run_pass(x2));
     on(2);
-    Prog x3; x3.load(nv->U3, bxp.rows_spec); l = x3.to_ortho(bxp);
+    Prog x3(so, 1); x3.load(nv->U3, bxp.rows_spec); l = x3.to_ortho(bxp);
     x3.store(nv->pres->vhat->d, l, ST_TRANS | ST_ACC, 1.0 / dt);
-    RET(run_pass(so, 1, x3));
+    RET(run_pass(x3));
   }
   RET(after(0, 1)); RET(after(0, 2));   // join
   on(0);

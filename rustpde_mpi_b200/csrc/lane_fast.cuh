@@ -219,73 +219,6 @@ __device__ __noinline__ void rfft_fast(const LaneProg& P, const LaneOp& op, doub
 }
 
 // ---------------------------------------------------------------------------------------------
-// banded mat-vec (see op_band): pairs p = q + t*TPL, t = 0..E; only t = 0 (first pair) and t = E (the pairs
-// beyond N/2) need range predicates.
-// ---------------------------------------------------------------------------------------------
-template <int E, int LN, int TPL>
-__device__ __noinline__ void band_fast(const LaneProg& P, const LaneOp& op, double* __restrict__ W) {
-  constexpr int CP = E + 1, PS = POff<LN, TPL>::v, M = E * TPL;
-  const int HP = P.LP >> 1;
-  const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
-  const int len_out = op.i0;
-  const int h0 = (int)(signed char)(op.i1 & 0xff), h1 = (int)(signed char)((op.i1 >> 8) & 0xff), h2 = (int)(signed char)((op.i1 >> 16) & 0xff);
-  const double2* __restrict__ c0 = (const double2*)op.p0;
-  const double2* __restrict__ c1 = (const double2*)op.p1;
-  const double2* __restrict__ c2 = (const double2*)op.p2;
-  double2* w2 = reinterpret_cast<double2*>(W) + 2 * l;
-  const double2 zero = d2(0.0, 0.0), one = d2(1.0, 1.0);
-  double2 y[CP];
-#pragma unroll
-  for (int t = 0; t < CP; t++) y[t] = zero;
-  auto term = [&](int h, const double2* __restrict__ c) {
-    const int hp = h >> 1;                 // -1 .. 2
-    const int bx = Lay<LN>::pix(q + hp);   // (q + hp = -1 gives a base that is only valid from t = 1 on)
-    const bool neg = (q + hp) < 0;
-    const int pl = q + M;
-    const bool okl = pl < HP && pl + hp < HP;
-    const double2 x0 = w2[neg ? 0 : bx], xl = w2[okl ? bx + E * PS : 0];
-    if (c) {
-      const double2 c0v = ldg(c + q), clv = ldg(c + (okl ? pl : 0));
-      if (!neg) y[0] = d2fma(c0v, x0, y[0]);
-#pragma unroll
-      for (int t = 1; t < E; t++) y[t] = d2fma(ldg(c + q + t * TPL), w2[bx + t * PS], y[t]);   // p + hp <= M + 1 < HP: in range
-      if (okl) y[E] = d2fma(clv, xl, y[E]);
-    } else {
-      if (!neg) { y[0].x += x0.x; y[0].y += x0.y; }
-#pragma unroll
-      for (int t = 1; t < E; t++) { const double2 x = w2[bx + t * PS]; y[t].x += x.x; y[t].y += x.y; }
-      if (okl) { y[E].x += xl.x; y[E].y += xl.y; }
-    }
-  };
-  if (h0 != 127) term(h0, c0);
-  if (h1 != 127) term(h1, c1);
-  if (h2 != 127) term(h2, c2);
-  __syncthreads();
-  const int bq = Lay<LN>::pix(q);
-  if (len_out >= 2 * M) {     // the usual case: only the pairs of t = E can reach len_out
-#pragma unroll
-    for (int t = 0; t < E; t++) w2[bq + t * PS] = y[t];
-  } else {
-#pragma unroll
-    for (int t = 0; t < E; t++) {
-      const int p = q + t * TPL;
-      double2 v = y[t];
-      if (2 * p >= len_out) v.x = 0.0;
-      if (2 * p + 1 >= len_out) v.y = 0.0;
-      w2[bq + t * PS] = v;
-    }
-  }
-  {
-    const int p = q + M;
-    double2 v = y[E];
-    if (2 * p >= len_out) v.x = 0.0;
-    if (2 * p + 1 >= len_out) v.y = 0.0;
-    if (p < HP) w2[bq + E * PS] = v;
-  }
-  __syncthreads();
-}
-
-// ---------------------------------------------------------------------------------------------
 // chunked recurrences: thread q owns pairs p0 + t, p0 = q*CP, t < CP (CP = E + 1 odd).  pix(p0 + t) is
 // base_even + c(t) for even t and base_odd + c(t) for odd t with compile-time c: two runtime bases per thread.
 // ---------------------------------------------------------------------------------------------
@@ -299,9 +232,9 @@ template <int LN> struct ChunkAddr {
   __device__ __forceinline__ int at(int t) const { return ((t & 1) ? bo : be) + Lay<LN>::pix(t); }
 };
 
-// Banded mat-vec with chunk ownership, streamed in place (OP_BANDC, set by the launcher): thread q owns the pairs
-// p0 + t like the recurrences below, reads every pair of W once and writes it once -- one read and one write traversal
-// of the lane group instead of one read per term plus the write of band_fast (the lane operators are bound by
+// Banded mat-vec with chunk ownership, streamed in place (OP_BANDC): thread q owns the pairs p0 + t like the recurrences
+// below, reads every pair of W once and writes it once -- one read and one write traversal of the lane group instead of
+// one read per term plus a write (the lane operators are bound by
 // shared-memory bandwidth, 128 B/clk: ~1k cycles per traversal of a 131 KB group).
 //   forward type  (i1 bit 0 = 0): y_p = k0 x_p + k1 x_{p+1} + k2 x_{p+2}   (pair offsets 0, +1, +2: S^T, MatVecFdma)
 //   backward type (i1 bit 0 = 1): y_p = k0 x_p + k1 x_{p-1}                (to_ortho stencil)

@@ -40,7 +40,8 @@
 enum LaneOpCode {
   OP_LOAD = 1,     // W = [W +|*] a * src           i0=len  i2=flags(LD_*)       p0=src (p1 = stencil coefficients)
   OP_STORE = 2,    // dst = [dst +] a * W            i0=len  i2=flags(ST_*)       p0=dst  (p1=peer table)
-  OP_BAND = 3,     // y_i = sum_m c_m[i] x_{i+o_m}   i0=len_out i1=packed offs i2=len_in  p0..p2 coef (null = 1, i1 byte=127: unused)
+  OP_BAND = 3,     // y_i = sum_m c_m[i] x_{i+o_m}   i0=len_out i1=packed offs i2=len_in  p0..p2 coef (null = 1, i1 byte=127: unused);
+                   //   generic geometry only (transform-sized lanes run OP_BANDC / OP_PREBAND)
   OP_DERIV = 4,    // Chebyshev d/dx of i0 coeffs, i1 times, times a
   OP_FDMA = 5,     // banded LU solve (fwd elim + back subst)  i0=len i2=flags(FD_*) p0=fl p1=inv_dia p2=u1 p3=u2 (fast geometry,
                    //   shared vectors: p0 = chunk-map table, LM_*)
@@ -52,8 +53,8 @@ enum LaneOpCode {
   OP_LANEMASK = 11,// lanes >= i0 zeroed
   OP_ZEROELEM = 12,// W[lane i0][pos i1] = 0 (global lane index)
   OP_SCALE = 13,   // W *= a
-  OP_PREBAND = 14, // an OP_BAND folded into the OP_FDMA that follows it (set by the launcher, fast geometry only): no-op here
-  OP_BANDC = 15,   // an OP_BAND in chunk-streaming form (set by the launcher, fast geometry only): see band_chunk
+  OP_PREBAND = 14, // an OP_BAND folded into the OP_FDMA that follows it (fast geometry only): no-op here
+  OP_BANDC = 15,   // an OP_BAND in chunk-streaming form (fast geometry only): see band_chunk
   OP_STEN3 = 16,   // ChebDirichletNeumann stencil (odd offsets): i1 = 0: y_j = x_j + a_{j-1} x_{j-1} + b_{j-2} x_{j-2} (to_ortho, S);
                    //   i1 = 1: y_k = x_k + a_k x_{k+1} + b_k x_{k+2} (S^T);  i0 = len_out, p0 = a, p1 = b (natural order)
   OP_DENSE = 18,   // dense mat-vec along the lane: y_k = sum_j M[k][j] x_j, i0 = n_out, i1 = n_in, p0 = M (row-major): the transforms
@@ -77,8 +78,8 @@ enum { ST_ACC = 1, ST_PLAIN = 2, ST_TRANS = 8, ST_PEER = 16,
                              // (operand of the eigen-transform GEMM, whose contraction runs over the rows); p1 = peer table
 enum { FD_PERLANE = 1, FD_NOU2 = 2,
        FD_PREBAND = 4 };   // the right-hand side is the banded mat-vec described by the preceding OP_PREBAND op
-// Chunk maps of an LU solve with shared coefficient vectors (set by the launcher on transform-sized lanes: OP_FDMA p0 = the
-// table, see fdma_fast_body).  Everything in it depends on the coefficients only, so the host computes it once.  double2 slot
+// Chunk maps of an LU solve with shared coefficient vectors (on transform-sized lanes OP_FDMA p0 = the table, see
+// fdma_fast_body).  Everything in it depends on the coefficients only, so the host computes it once.  double2 slot
 // [s][q] of the thread that owns pairs q*CP + t (both parities), s = LM_x * CP + t for the per-pair entries:
 //   LM_FL: fl   LM_ID: id   LM_U1: u1 * id   LM_U2: u2 * id
 //   LM_WA, LM_WB: weight of y_t in x_{p0} and x_{p0+1} of the chunk's back-substitution map (entered with zero state)
@@ -1312,7 +1313,7 @@ __global__ void B2_LB lane_kernel(const __grid_constant__ LaneProg Pp) {
         else store_threads<LN>(P, op, sv, g, gl, lb);
         break;
       case OP_BAND:
-        if constexpr (TPLC > 0) band_fast<E, LN, TPLC>(P, op, W); else op_band<E + 1, LN>(P, op, W);
+        if constexpr (TPLC == 0) op_band<E + 1, LN>(P, op, W);
         break;
       case OP_DERIV:
         if constexpr (TPLC > 0) deriv_fast<E, LN, TPLC>(P, op, W, scratch); else op_deriv<E + 1, LN>(P, op, W, scratch);
