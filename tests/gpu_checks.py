@@ -85,14 +85,147 @@ def check_from_ortho(k0, n0, k1, n1, seed=4):
     return relerr(fg.vhat, fo.vhat)
 
 
-def check_gradient(k0, n0, k1, n1, deriv, scale=(1.5, 1.0), seed=5):
-    fo, fg = mk(k0, n0, k1, n1)
+def decaying_spec(fo, seed):
+    """random spectrum decaying like 1 / (1 + i + j)^2: physically sized, so that derivatives stay O(1)"""
     a = rand_spec(fo, seed)
-    # physically sized spectrum: decay so that derivatives stay O(1)
     i = np.arange(a.shape[0])[:, None]; j = np.arange(a.shape[1])[None, :]
-    a = a / (1.0 + i + j) ** 2
+    return a / (1.0 + i + j) ** 2
+
+
+def check_gradient(k0, n0, k1, n1, deriv, scale=(1.5, 1.0), seed=5):
+    """``scale=None`` runs the unscaled path (a NULL scale through the C ABI)"""
+    fo, fg = mk(k0, n0, k1, n1)
+    a = decaying_spec(fo, seed)
     fo.vhat = a.copy(); fg.vhat = a
     return relerr(fg.gradient(deriv, scale).get(), fo.gradient(deriv, scale))
+
+
+def perturbed(a, seed):
+    """``a`` changed in the last bit: multiplied by 1 + 4e-16 N(0,1) (the conditioning yardstick's input)"""
+    return a * (1.0 + 4e-16 * np.random.default_rng(seed).standard_normal(a.shape))
+
+
+def check_gradient_yardstick(k0, n0, k1, n1, deriv, scale=(1.5, 1.0), seed=5):
+    """check_gradient's error AND the yardstick = the oracle against itself on the same spectrum changed in the last bit"""
+    fo, fg = mk(k0, n0, k1, n1)
+    a = decaying_spec(fo, seed)
+    fo.vhat = a.copy(); fg.vhat = a
+    ref = fo.gradient(deriv, scale)
+    err = relerr(fg.gradient(deriv, scale).get(), ref)
+    fo.vhat = perturbed(a, 1000 + seed)
+    return err, relerr(fo.gradient(deriv, scale), ref)
+
+
+# ---- the state a call leaves behind: padding and reused outputs ----
+def borrowed(field, which):
+    """non-owning DeviceArray over a field's ``v`` (which = 0) or ``vhat`` (1)"""
+    import ctypes as C
+
+    from rustpde_mpi_b200._lib import check, lib
+
+    h = C.c_void_p()
+    check(lib().b2_field_array(field._h, which, C.byref(h)))
+    return b2.DeviceArray(field.space, b2.PHYSICAL if which == 0 else b2.SPECTRAL, handle=h, owner=False)
+
+
+def padding_excess(arr):
+    """|norm of the whole padded device array - norm of its logical elements| / the latter: nonzero when a store left
+    anything in the padding (which the reductions over the padded array, norm2 / axpy / combine, would then see)"""
+    host = float(np.linalg.norm(arr.get().ravel()))
+    return abs(arr.norm() - host) / max(host, 1e-300)
+
+
+def nan_fill(arr):
+    """every logical element NaN (set() zeroes the padding before it uploads): an operator that leaves one unwritten fails"""
+    shape = arr.local_shape()
+    cx = arr.space.shape(arr.kind)[1]
+    arr.set(np.full(shape, complex(np.nan, np.nan) if cx else np.nan))
+    return arr
+
+
+SEQ_DERIVS = ((1, 0), (0, 1), (2, 0), (0, 2), (1, 1), (3, 0), (0, 3))
+CD, CN, R2C, C2C = 1, 2, 4, 5
+
+
+def call_sequence(k0, n0, k1, n1, seed=11):
+    """Generator over one space, one Field2, one ORTHO and one SPECTRAL output reused throughout; every destination is
+    NaN-filled before the operator that writes it.  Yields (step, relative error against the oracle, padding_excess of the
+    destination) after each step: forward, to_ortho, from_ortho, backward, gradients at SEQ_DERIVS (scaled and unscaled),
+    dealias, backward, forward, then HholtzAdi / Poisson / Hholtz interleaved, each twice into the same output, and a last
+    to_ortho after the solves (they share the space's scratch with the field operators)."""
+    fo, fg = mk(k0, n0, k1, n1)
+    v, vhat = borrowed(fg, 0), borrowed(fg, 1)
+    out, sout = b2.DeviceArray(fg.space, b2.ORTHO), b2.DeviceArray(fg.space, b2.SPECTRAL)
+    rng = np.random.default_rng(seed)
+
+    fo.v = rand_phys(fo, rng, "uniform"); fg.v = fo.v
+    nan_fill(vhat); fg.forward(); fo.forward()
+    yield "forward", relerr(fg.vhat, fo.vhat), padding_excess(vhat)
+    nan_fill(out); fg.to_ortho(out=out); ref = fo.to_ortho()
+    yield "to_ortho", relerr(out.get(), ref), padding_excess(out)
+    nan_fill(vhat); fg.from_ortho(out); fo.from_ortho(ref)
+    yield "from_ortho", relerr(fg.vhat, fo.vhat), padding_excess(vhat)
+    nan_fill(v); fg.backward(); fo.backward()
+    yield "backward", relerr(fg.v, fo.v), padding_excess(v)
+
+    a = decaying_spec(fo, seed)
+    fo.vhat = a.copy(); fg.vhat = a
+    for d in SEQ_DERIVS:
+        for scale in ((1.5, 0.5), None):
+            nan_fill(out); fg.gradient(d, scale, out=out)
+            yield f"gradient{d}{'' if scale else '-unscaled'}", relerr(out.get(), fo.gradient(d, scale)), padding_excess(out)
+    if k0 != C2C:   # the 2/3 rule is defined for r2c / Chebyshev mode order only
+        fg.dealias(); o.dealias(fo.vhat)
+        yield "dealias", relerr(fg.vhat, fo.vhat), padding_excess(vhat)
+    nan_fill(v); fg.backward(); fo.backward()
+    yield "backward", relerr(fg.v, fo.v), padding_excess(v)
+    nan_fill(vhat); fg.forward(); fo.forward()
+    yield "forward", relerr(fg.vhat, fo.vhat), padding_excess(vhat)
+
+    solvers = []
+    if 0 not in (k0, k1):
+        solvers.append(("hholtz_adi", o.HholtzAdi(fo, [0.02, 0.03]), b2.HholtzAdi(fg, [0.02, 0.03])))
+    # Poisson / Hholtz: the lane kernel runs their per-row LU along axis 1; a long confined axis 0 only adds the host LAPACK
+    # eigendecomposition (tens of seconds beyond 1025 points)
+    if k0 in (CD, CN, R2C) and k1 in (CD, CN) and (k0 == R2C or n0 <= 1025):
+        eig = b2.poisson_eig(k0, n0, 1.0) if k0 != R2C else None
+        solvers.append(("poisson", o.Poisson(fo, [1.0, 1.0], eig=eig), b2.Poisson(fg, [1.0, 1.0])))
+        eig = b2.hholtz_eig(k0, n0, 0.37) if k0 != R2C else None
+        solvers.append(("hholtz", o.Hholtz(fo, [0.37, 1.3], eig=eig), b2.Hholtz(fg, [0.37, 1.3])))
+    if solvers:
+        sh, cx = fg.space.shape(b2.ORTHO)
+        rhs = rng.standard_normal(sh) + (1j * rng.standard_normal(sh) if cx else 0.0)
+        out.set(rhs)
+        for rep in range(2):
+            for name, so, sg in solvers:
+                nan_fill(sout); sg.solve(out, out=sout)
+                xo, xg = so.solve(rhs), sout.get()
+                if name == "poisson":
+                    xo[0, 0] = 0; xg[0, 0] = 0   # the shifted-singular mode is removed by the caller (navier_eq.rs:161)
+                yield f"{name}#{rep}", relerr(xg, xo), padding_excess(sout)
+        nan_fill(out); fg.to_ortho(out=out)
+        yield "to_ortho", relerr(out.get(), fo.to_ortho()), padding_excess(out)
+
+
+def run_sequences(*spaces, seed=11):
+    """Run the call sequences of several spaces in one context, alternating step by step (every step switches the space and
+    with it the lane-kernel instances, the staging buffer size and the solver workspaces).  Returns {space: [(step, err,
+    padding_excess)]}."""
+    gens = {sp: call_sequence(*sp, seed=seed) for sp in spaces}
+    res = {sp: [] for sp in spaces}
+    while gens:
+        for sp in list(gens):
+            try:
+                res[sp].append(next(gens[sp]))
+            except StopIteration:
+                del gens[sp]
+    return res
+
+
+def sequence_failures(res, pad_tol=1e-13):
+    """the steps of run_sequences' result over TOL or the padding bound (NaN fails both)"""
+    return {f"{sp}:{i}:{step}": (e, p) for sp, steps in res.items() for i, (step, e, p) in enumerate(steps)
+            if not (e < TOL and p < pad_tol)}
 
 
 def check_hholtz(k0, n0, k1, n1, c=(0.02, 0.03), seed=6):
@@ -131,6 +264,45 @@ def check_hholtz_tensor(k0, n0, k1, n1, c=(0.37, 1.3), seed=9):
     if fo.vhat.dtype == np.complex128:
         rhs = rhs + 1j * rng.standard_normal(sh)
     return relerr(hg.solve(rhs).get(), ho.solve(rhs))
+
+
+def bench_coefficients(ra, dt, aspect=1.0, pr=1.0):
+    """the Helmholtz coefficients of a Navier2D step, as b2_navier2d_create computes them: (c_velocity, c_temperature) with
+    c = (dt nu / aspect^2, dt nu) and nu = sqrt(pr / (ra / 8)), ka = sqrt(1 / (ra / 8 pr)) (height 2, functions.rs:12-21)"""
+    nu = np.sqrt(pr / (ra / 2.0 ** 3)); ka = np.sqrt(1.0 / ((ra / 2.0 ** 3) * pr))
+    return (dt * nu / aspect ** 2, dt * nu), (dt * ka / aspect ** 2, dt * ka)
+
+
+def check_solver_yardstick(name, k0, n0, k1, n1, c, seed=8):
+    """``name`` in hholtz_adi / poisson / hholtz on a white-noise right-hand side: the error against the oracle AND the
+    yardstick = the oracle against itself on the right-hand side changed in the last bit (x (1 + 4e-16 N(0,1)))"""
+    fo, fg = mk(k0, n0, k1, n1)
+    if name == "hholtz_adi":
+        so, sg = o.HholtzAdi(fo, list(c)), b2.HholtzAdi(fg, list(c))
+    else:
+        eig = (b2.poisson_eig if name == "poisson" else b2.hholtz_eig)(k0, n0, c[0]) if k0 in (CD, CN) else None
+        so, sg = (o.Poisson, o.Hholtz)[name == "hholtz"](fo, list(c), eig=eig), (b2.Poisson, b2.Hholtz)[name == "hholtz"](fg, list(c))
+    sh, cx = fg.space.shape(b2.ORTHO)
+    rng = np.random.default_rng(seed)
+    rhs = rng.standard_normal(sh) + (1j * rng.standard_normal(sh) if cx else 0.0)
+    xo, xp, xg = so.solve(rhs), so.solve(perturbed(rhs, 1000 + seed)), sg.solve(rhs).get()
+    if name == "poisson":
+        for x in (xo, xp, xg):
+            x[0, 0] = 0   # the shifted-singular mode is removed by the caller (navier_eq.rs:161)
+    return relerr(xg, xo), relerr(xp, xo)
+
+
+def check_navier_padding(nav):
+    """padding_excess of v and vhat of every state and work field of a CUDA Navier2D, and div_norm() against the host norm
+    of div(): {name: value}"""
+    out = {}
+    for name in ("temp", "velx", "vely", "pres", "pseu"):
+        f = getattr(nav, name)
+        for which in (0, 1):
+            out[f"{name}.{'vhat' if which else 'v'}"] = padding_excess(borrowed(f, which))
+    d = float(np.linalg.norm(nav.div().ravel()))
+    out["div_norm"] = abs(nav.div_norm() - d) / max(d, 1e-300)
+    return out
 
 
 def make_navier_pair(nx, ny, ra, pr, dt, aspect, periodic, init="modes", bc="rbc"):
