@@ -268,19 +268,6 @@ static std::vector<double> scan_layout(const std::vector<double>& v, int C, int 
   return o;
 }
 
-// Coefficient vector of a banded mat-vec: natural order (OP_BAND, generic geometry) and its scan-layout copy for the chunking
-// (C, TPL) it was built for (OP_BANDC / OP_PREBAND, transform-sized lanes).
-struct BandVec {
-  DVecD nat, scan;
-  int C = 0, TPL = 0;
-  int upload(const std::vector<double>& v, int C_, int TPL_) {
-    C = C_; TPL = TPL_;
-    RET(nat.upload(v));
-    return scan.upload(scan_layout(v, C, TPL));
-  }
-  void release() { nat.release(); scan.release(); }
-};
-
 // LU coefficients of a banded solve (OP_FDMA) in scan layout for the chunking (C, TPL) they were built for: one set shared by
 // every lane, with the chunk-map table that the compile-time-geometry solve runs on (map), or one set per lane (perlane, the
 // Poisson per-row LU: [lane group][t][q][lane]).  u2 absent: FD_NOU2.
@@ -341,15 +328,17 @@ struct Base1 {
   bool c2c = false;                        // FourierC2c: complex physical values, n modes in FFT order (k = 0 .. n/2-1, -n/2 .. -1)
   int rows_phys = 0, rows_spec = 0, rows_ortho = 0;  // real rows along this axis (complex => 2 per mode)
   int N = 0;                                          // transform size (n-1 Chebyshev, n Fourier)
-  std::vector<double> s2;                             // stencil: ortho_k = c_k + s2[k-2] c_{k-2}
-  BandVec bsten, bs2;                                 // composite: stencil of to_ortho (bsten[j] = s2[j-2]), S^T of from_ortho
-  BandVec bd, bu1, bu2;                               // composite / cdn: MatVecFdma of the preconditioner pinv
+  std::vector<double> s2;                             // stencil: ortho_k = c_k + s2[k-2] c_{k-2} (the lane kernel forms it: band_coef.cuh)
   LuDev tlu;                                          // composite: from_ortho solve (S^T S) c = S^T o
   DVecD d_tw, d_tw2, d_isin;
   std::vector<double> ca, cb;                         // cdn stencil: ortho_k = c_k + ca[k-1] c_{k-1} + cb[k-2] c_{k-2}
   DVecD d_dfwd, d_dbwd; bool dense_tr = false;       // transform sizes the FFT core does not handle: dense matrices (OP_DENSE)
   DVecD d_ca, d_cb, d_pent; int pent_L = 0;            // cdn: stencil vectors, packed PdmaPlus2 LU of S^T S (from_ortho)
 
+  // coefficient families of the banded mat-vecs (band_coef.cuh: the lane kernel forms s2 and pv itself)
+  bool neumann() const { return kind == B2_CHEB_NEUMANN; }
+  int sten_family() const { return neumann() ? BC_STEN_N : BC_STEN_D; }   // to_ortho stencil, s2[j-2] at element j
+  int s2_family() const { return neumann() ? BC_S2_N : BC_S2_D; }         // S^T of from_ortho, s2[k] at element k
   // B2 = laplace_inv (SURVEY 8a row G); pv(i, off) = (laplace_inv_eye . laplace_inv)[i, i+off]
   double pv(int i, int off) const {
     const int r = i + 2;
@@ -395,7 +384,6 @@ struct Base1 {
   int init(int C, int TPL);   // device vectors; (C, TPL) = chunking of the passes whose lanes run along this axis
   int lay_C = 1, lay_TPL = 1;
   void release() {
-    for (BandVec* v : {&bsten, &bs2, &bd, &bu1, &bu2}) v->release();
     tlu.release();
     for (DVecD* v : {&d_tw, &d_tw2, &d_isin, &d_ca, &d_cb, &d_pent, &d_dfwd, &d_dbwd}) v->release();
   }
@@ -440,10 +428,6 @@ int Base1::init(int C, int TPL) {
   lay_C = C; lay_TPL = TPL;
   const int L = roundup(std::max(rows_phys, rows_ortho) + 8, 4) + 64;  // generous coefficient-vector length
   if (composite) {
-    std::vector<double> sten2(L, 0.0), s2v(L, 0.0);
-    for (int i = 2; i < n; i++) sten2[i] = s2[i - 2];
-    for (int k = 0; k < m; k++) s2v[k] = s2[k];
-    RET(bsten.upload(sten2, C, TPL)); RET(bs2.upload(s2v, C, TPL));
     // from_ortho: (S^T S) c = S^T o, tridiagonal at offsets (-2,0,2) (SURVEY A.2)
     Diags t(m);
     for (int k = 0; k < m; k++) {
@@ -451,15 +435,6 @@ int Base1::init(int C, int TPL) {
       if (k + 2 < m) { t.low[k] = s2[k]; t.up1[k] = s2[k]; }
     }
     RET(upload_lu(sweep(t), false, C, TPL, &tlu));
-  }
-  if (composite || cdn) {   // MatVecFdma of the preconditioner pinv (src/solver/matvec.rs:177-203), the same for every composite base
-    std::vector<double> vd(L, 0.0), vu1(L, 0.0), vu2(L, 0.0);
-    for (int i = 0; i < m; i++) {
-      vd[i] = pv(i, 0);
-      if (i < m - 2) vu1[i] = pv(i, 2);
-      if (i < m - 4) vu2[i] = pv(i, 4);
-    }
-    RET(bd.upload(vd, C, TPL)); RET(bu1.upload(vu1, C, TPL)); RET(bu2.upload(vu2, C, TPL));
   }
   if (cdn) {
     std::vector<double> a(L, 0.0), b(L, 0.0);
@@ -691,22 +666,19 @@ struct Prog {
   }
   void load(const double* src, int len, double a = 1.0, int flags = 0, int i1 = 0) { LaneOp* o = add(OP_LOAD); o->p0 = src; o->i0 = len; o->a = a; o->i2 = flags; o->i1 = i1; }
   void store(double* dst, int len, int flags, double a = 1.0, int i1 = 0) { LaneOp* o = add(OP_STORE); o->p0 = dst; o->i0 = len; o->a = a; o->i2 = flags; o->i1 = i1; }
-  // Banded mat-vec y_i = k0_i x_i + k1_i x_{i+o1} + k2_i x_{i+4}: o1 = +2, or -2 for the to_ortho stencil; k0 null = 1, k2
-  // null = no term.  Transform-sized lanes run it in chunk-streaming form (OP_BANDC, band_chunk: one read and one write
-  // traversal of the lane group) on the scan-layout copies, or fold it into the LU solve emitted next (OP_PREBAND).
-  void band(int len_out, int len_in, const BandVec* k0, int o1, const BandVec& k1, const BandVec* k2 = nullptr, bool fold = false) {
-    const BandVec* k[3] = {k0, &k1, k2};
-    LaneOp* o = add(OP_BAND); o->i0 = len_out; o->i2 = len_in; o->i1 = pack_offs(0, o1, k2 ? 4 : 127);
-    const void** cp[3] = {&o->p0, &o->p1, &o->p2};
-    for (int m = 0; m < 3; m++) {
-      if (!k[m]) continue;
-      if (c.fast && !chunked(k[m]->C, k[m]->TPL, "band coefficients")) return;
-      *cp[m] = c.fast ? k[m]->scan.d : k[m]->nat.d;
-    }
+  // Banded mat-vec y_i = k0_i x_i + k1_i x_{i+o1} + k2_i x_{i+4} of a base of size n: o1 = +2, or -2 for the to_ortho
+  // stencil; k0..k2 are coefficient families (band_coef.cuh), formed by the lane kernel.  Transform-sized lanes run it in
+  // chunk-streaming form (OP_BANDC, band_chunk: one read and one write traversal of the lane group), or fold it into the LU
+  // solve emitted next (OP_PREBAND); both have one compile-time instance per term combination, the ones emitted here.
+  void band(int len_out, int n, int k0, int o1, int k1, int k2 = BC_ABSENT, bool fold = false) {
+    const int terms = B2_BAND_TERMS(k0, k1, k2);
+    const bool known = (o1 < 0) ? (terms == B2_BAND_TERMS(BC_UNIT, BC_STEN_D, BC_ABSENT) || terms == B2_BAND_TERMS(BC_UNIT, BC_STEN_N, BC_ABSENT))
+                                : (terms == B2_BAND_TERMS(BC_UNIT, BC_S2_D, BC_ABSENT) || terms == B2_BAND_TERMS(BC_UNIT, BC_S2_N, BC_ABSENT) ||
+                                   terms == B2_BAND_TERMS(BC_PV0, BC_PV2, BC_PV4));
+    if (!known) { err = fail(B2_ERR_ARG, "banded mat-vec with a term combination the lane kernel has no instance of"); return; }
+    LaneOp* o = add(OP_BAND); o->i0 = len_out; o->i1 = pack_offs(0, o1, k2 ? 4 : 127); o->i2 = band_fams(k0, k1, k2, n);
     if (!c.fast) return;
-    if (fold) { o->code = OP_PREBAND; return; }
-    o->code = OP_BANDC;   // term flags: 1 unit coefficient, 2 vector (band_chunk)
-    o->i1 = (o1 < 0 ? 1 : 0) | ((k0 ? 2 : 1) << 2) | (2 << 4) | ((k2 ? 2 : 0) << 6);
+    o->code = fold ? OP_PREBAND : OP_BANDC;
   }
   void deriv(int n, int times, double scale) { LaneOp* o = add(OP_DERIV); o->i0 = n; o->i1 = times; o->a = scale; }
   // LU solve; shared vectors run on their chunk-map table on transform-sized lanes (fdma_fast_body)
@@ -718,9 +690,9 @@ struct Prog {
   // LU solve with shared vectors of the mat-vec (k0, k1 at +2, k2 at +4) of W.  On E <= 8 transform-sized lanes the solve forms
   // that right-hand side itself from the OP_PREBAND op just before it (fdma_fast_body reads it there).  On E = 16 the extra
   // coefficient streams cost more than the saved pass (0.14 ms per step slower on C4, H100 SXM at 400 W), so it stays OP_BANDC.
-  void band_solve(int len, int len_in, const BandVec* k0, const BandVec& k1, const BandVec* k2, const LuDev& lu) {
+  void band_solve(int len, int n, int k0, int k1, int k2, const LuDev& lu) {
     const bool fold = c.fast && c.E <= 8;
-    band(len, len_in, k0, 2, k1, k2, fold);
+    band(len, n, k0, 2, k1, k2, fold);
     fdma(len, lu, fold ? FD_PREBAND : 0);
   }
   void dense(int n_out, int n_in, const double* M) { LaneOp* o = add(OP_DENSE); o->i0 = n_out; o->i1 = n_in; o->p0 = M; }
@@ -748,9 +720,9 @@ struct Prog {
       // staging slots took longer per lane group than the zero-copy load and band_chunk together).
       LaneOp* lo = p.nops ? &p.ops[p.nops - 1] : nullptr;
       if (!c.fast && lo && lo->code == OP_LOAD && !(lo->i2 & (LD_PLAIN | LD_STENCIL | LD_ACC | LD_MUL)) && lo->i0 == b.m) {
-        lo->i2 |= LD_STENCIL; lo->p1 = b.bsten.nat.d; lo->i0 = b.n;
+        lo->i2 |= LD_STENCIL | (b.neumann() ? LD_NEUMANN : 0); lo->i0 = b.n;
       } else {
-        band(b.n, b.m, nullptr, -2, b.bsten);
+        band(b.n, b.n, BC_UNIT, -2, b.sten_family());
       }
       return b.n;
     }
@@ -759,7 +731,7 @@ struct Prog {
   }
   int from_ortho(const Base1& b) {
     if (b.cdn) { sten3(b.m, 1, b); pdma(b.m, b.d_pent.d, b.pent_L); return b.m; }
-    if (b.composite) { band_solve(b.m, b.n, nullptr, b.bs2, nullptr, b.tlu); return b.m; }
+    if (b.composite) { band_solve(b.m, b.n, BC_UNIT, b.s2_family(), BC_ABSENT, b.tlu); return b.m; }
     return b.rows_spec;
   }
   int deriv_axis(const Base1& b, int d, double sc) {  // on ortho coefficients; sc = 1/scale^d
@@ -779,11 +751,10 @@ struct Prog {
     LaneOp* o = add(OP_LOAD); o->p0 = src; o->a = a;
     o->i0 = b.rows_ortho;
     if (b.cdn) err = fail(B2_ERR_UNSUPPORTED, "stencil-on-load is pair-structured (ChebDirichletNeumann uses OP_STEN3)");
-    o->i2 = (acc ? LD_ACC : 0) | (b.composite ? LD_STENCIL : 0);
-    o->p1 = b.bsten.nat.d;
+    o->i2 = (acc ? LD_ACC : 0) | (b.composite ? LD_STENCIL | (b.neumann() ? LD_NEUMANN : 0) : 0);
   }
   int matvec(const Base1& b) {          // MatVecFdma with pinv (Chebyshev axes only)
-    if (b.composite || b.cdn) { band(b.m, b.n, &b.bd, 2, b.bu1, &b.bu2); return b.m; }
+    if (b.composite || b.cdn) { band(b.m, b.n, BC_PV0, 2, BC_PV2, BC_PV4); return b.m; }
     return b.rows_spec;
   }
 };
@@ -1407,7 +1378,7 @@ static int poisson_solve(b2_solver* s, const double* in, double* out, bool zero0
 // one axis of HholtzAdi: precondition (MatVecFdma) + banded / diagonal solve
 static void emit_hh_axis(Prog& p, const b2_solver* s, int ax) {
   const Base1& b = s->sp->b[ax];
-  if (b.composite) { p.band_solve(b.m, b.n, &b.bd, b.bu1, &b.bu2, s->lu[ax]); return; }
+  if (b.composite) { p.band_solve(b.m, b.n, BC_PV0, BC_PV2, BC_PV4, s->lu[ax]); return; }
   p.matvec(b);
   if (b.cdn) p.pdma(b.m, s->pd[ax].d, s->pd_L[ax]);   // hholtz_adi.rs:64
   else p.scalevec(b.rows_spec, s->sd[ax].d, 1);

@@ -236,41 +236,32 @@ template <int LN> struct ChunkAddr {
 // below, reads every pair of W once and writes it once -- one read and one write traversal of the lane group instead of
 // one read per term plus a write (the lane operators are bound by
 // shared-memory bandwidth, 128 B/clk: ~1k cycles per traversal of a 131 KB group).
-//   forward type  (i1 bit 0 = 0): y_p = k0 x_p + k1 x_{p+1} + k2 x_{p+2}   (pair offsets 0, +1, +2: S^T, MatVecFdma)
-//   backward type (i1 bit 0 = 1): y_p = k0 x_p + k1 x_{p-1}                (to_ortho stencil)
-// term flags, 2 bits each from bit 2: 0 absent, 1 unit coefficient, 2 scan-layout vector ([t][q]) in p0 / p1 / p2.
-template <int E, int LN, int TPL>
-__device__ __noinline__ void band_chunk(const LaneProg& P, const LaneOp& op, double* __restrict__ W) {
+//   forward type  (term 1 at offset +2): y_p = k0 x_p + k1 x_{p+1} + k2 x_{p+2}   (pair offsets 0, +1, +2: S^T, MatVecFdma)
+//   backward type (term 1 at offset -2): y_p = k0 x_p + k1 x_{p-1}                (to_ortho stencil)
+// The coefficients are formed in registers from their families (band_coef.cuh): no coefficient loads.
+template <int E, int LN, int TPL, int F0, int F1, int F2>
+__device__ __forceinline__ void band_chunk_body(const LaneProg& P, const LaneOp& op, double* __restrict__ W) {
   constexpr int CP = E + 1;
+  constexpr bool BACKWARD = F1 == BC_STEN_D || F1 == BC_STEN_N;
   const int HP = P.LP >> 1;
   const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
   double2* w2 = reinterpret_cast<double2*>(W) + 2 * l;
   const int p0 = q * CP;
   const ChunkAddr<LN> ca(p0);
   const int tmax = HP - p0;                                     // t < tmax: the pair exists in W
-  const int len_out = op.i0;
+  const int len_out = op.i0, n = band_n(op.i2);
   const int tx = (len_out - 2 * p0 + 1) >> 1, ty = (len_out - 2 * p0) >> 1;   // t < tx: element 2p < len_out; t < ty: 2p+1 < len_out
   const double2 zero = d2(0.0, 0.0);
-  const double2* cp[3] = {(const double2*)op.p0, (const double2*)op.p1, (const double2*)op.p2};
-  const double2* any = cp[0] ? cp[0] : (cp[1] ? cp[1] : cp[2]);
-  double wl[3], ad[3];                                          // coefficient = loaded * wl + ad (loads stay unconditional)
-#pragma unroll
-  for (int m = 0; m < 3; m++) {
-    const int f = (op.i1 >> (2 + 2 * m)) & 3;
-    wl[m] = (f == 2) ? 1.0 : 0.0; ad[m] = (f == 1) ? 1.0 : 0.0;
-    cp[m] = ((f == 2) ? cp[m] : any) + q;
-  }
-  if (!(op.i1 & 1)) {
+  BandPairs<F0, F1, F2> cf(n, 2 * p0);
+  if constexpr (!BACKWARD) {
     const double2 hA = (CP < tmax) ? w2[ca.at(CP)] : zero, hB = (CP + 1 < tmax) ? w2[ca.at(CP + 1)] : zero;
     __syncthreads();
     double2 x0 = (0 < tmax) ? w2[ca.at(0)] : zero, x1 = (1 < tmax) ? w2[ca.at(1)] : zero;
 #pragma unroll
     for (int t = 0; t < CP; t++) {
       const double2 x2 = (t + 2 < CP) ? ((t + 2 < tmax) ? w2[ca.at(t + 2 < CP ? t + 2 : 0)] : zero) : (t + 2 == CP ? hA : hB);
-      const double2 l0 = ldg(cp[0] + t * TPL), l1 = ldg(cp[1] + t * TPL), l2 = ldg(cp[2] + t * TPL);
-      const double2 k0 = d2(fma(l0.x, wl[0], ad[0]), fma(l0.y, wl[0], ad[0]));
-      const double2 k1 = d2(fma(l1.x, wl[1], ad[1]), fma(l1.y, wl[1], ad[1]));
-      const double2 k2 = d2(fma(l2.x, wl[2], ad[2]), fma(l2.y, wl[2], ad[2]));
+      double2 k0, k1, k2;
+      cf.at(2 * (p0 + t), k0, k1, k2);
       double2 b = d2fma(k0, x0, d2fma(k1, x1, d2(k2.x * x2.x, k2.y * x2.y)));
       if (t >= tx) b.x = 0.0;
       if (t >= ty) b.y = 0.0;
@@ -284,9 +275,8 @@ __device__ __noinline__ void band_chunk(const LaneProg& P, const LaneOp& op, dou
 #pragma unroll
     for (int t = CP - 1; t >= 0; t--) {
       const double2 xm = (t > 0) ? ((t - 1 < tmax) ? w2[ca.at(t > 0 ? t - 1 : 0)] : zero) : hP;
-      const double2 l0 = ldg(cp[0] + t * TPL), l1 = ldg(cp[1] + t * TPL);
-      const double2 k0 = d2(fma(l0.x, wl[0], ad[0]), fma(l0.y, wl[0], ad[0]));
-      const double2 k1 = d2(fma(l1.x, wl[1], ad[1]), fma(l1.y, wl[1], ad[1]));
+      double2 k0, k1, k2;
+      cf.at(2 * (p0 + t), k0, k1, k2);
       double2 b = d2fma(k0, x0, d2(k1.x * xm.x, k1.y * xm.y));
       if (t >= tx) b.x = 0.0;
       if (t >= ty) b.y = 0.0;
@@ -295,6 +285,17 @@ __device__ __noinline__ void band_chunk(const LaneProg& P, const LaneOp& op, dou
     }
   }
   __syncthreads();
+}
+// the term combinations Prog::band emits (checked there): one compile-time instance each, chosen once per op
+template <int E, int LN, int TPL>
+__device__ __noinline__ void band_chunk(const LaneProg& P, const LaneOp& op, double* __restrict__ W) {
+  switch (band_terms(op.i2)) {
+    case B2_BAND_TERMS(BC_UNIT, BC_STEN_D, BC_ABSENT): band_chunk_body<E, LN, TPL, BC_UNIT, BC_STEN_D, BC_ABSENT>(P, op, W); break;
+    case B2_BAND_TERMS(BC_UNIT, BC_STEN_N, BC_ABSENT): band_chunk_body<E, LN, TPL, BC_UNIT, BC_STEN_N, BC_ABSENT>(P, op, W); break;
+    case B2_BAND_TERMS(BC_UNIT, BC_S2_D, BC_ABSENT): band_chunk_body<E, LN, TPL, BC_UNIT, BC_S2_D, BC_ABSENT>(P, op, W); break;
+    case B2_BAND_TERMS(BC_UNIT, BC_S2_N, BC_ABSENT): band_chunk_body<E, LN, TPL, BC_UNIT, BC_S2_N, BC_ABSENT>(P, op, W); break;
+    case B2_BAND_TERMS(BC_PV0, BC_PV2, BC_PV4): band_chunk_body<E, LN, TPL, BC_PV0, BC_PV2, BC_PV4>(P, op, W); break;
+  }
 }
 
 template <int E, int LN, int TPL>
@@ -338,7 +339,7 @@ __device__ __noinline__ void deriv_fast(const LaneProg& P, const LaneOp& op, dou
 // weighted sum of the chunk's y (2 FMA per pair and parity instead of composing a 2x2 affine map per pair), and the solve does
 // not multiply by id.  The per-lane arrays stream from HBM (one set per lane), where a table of 6 vectors instead of 4 would
 // cost more traffic than the arithmetic it saves, so they keep the composing form.
-template <int E, int LN, int TPL, bool PERLANE, bool PREBAND>
+template <int E, int LN, int TPL, bool PERLANE, bool PREBAND, class BAND = BandPairs<BC_ABSENT, BC_ABSENT, BC_ABSENT>>
 __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& op, double* __restrict__ W, int gl, int lb, void* scratch) {
   constexpr int CP = E + 1, CS = PERLANE ? 4 * TPL : TPL;
   constexpr bool MAPS = !PERLANE;
@@ -376,33 +377,19 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
     double2 A = d2(1.0, 1.0), B = zero;
     if constexpr (PREBAND) {
       // The right-hand side is a banded mat-vec of what is in W: b_p = c0_p x_p + c1_p x_{p+1} + c2_p x_{p+2}
-      // (pair offsets 0, +1, +2; a null coefficient vector = 1; scan-layout vectors [t][q]).  It is formed here, on the
+      // (pair offsets 0, +1, +2, coefficients of the families BAND, formed in registers).  It is formed here, on the
       // fly, and written back in place; the two pairs after the chunk are read before anybody writes.
       const LaneOp& bop = *(&op - 1);
-      // every term loads unconditionally (absent / unit coefficients read the LU vector instead and are blended
-      // to 0 / 1 afterwards), so that the 3 x CP coefficient loads can all be in flight at once
-      const double2* cf[3] = {cfl, cfl, cfl};
-      double wl[3] = {0.0, 0.0, 0.0}, ad[3] = {0.0, 0.0, 0.0};   // coefficient = loaded * wl + ad
-#pragma unroll
-      for (int m = 0; m < 3; m++) {
-        const int h = (int)(signed char)((bop.i1 >> (8 * m)) & 0xff);
-        const double2* cp = (const double2*)(m == 0 ? bop.p0 : (m == 1 ? bop.p1 : bop.p2));
-#pragma unroll
-        for (int k = 0; k < 3; k++)
-          if (h == 2 * k) { if (cp) { cf[k] = cp + q; wl[k] = 1.0; } else ad[k] = 1.0; }
-      }
+      BAND cf(band_n(bop.i2), 2 * p0);
       const double2 hA = (CP < tmax) ? w2[ca.at(CP)] : zero, hB = (CP + 1 < tmax) ? w2[ca.at(CP + 1)] : zero;
       __syncthreads();
       double2 x0 = (0 < tmax) ? w2[ca.at(0)] : zero, x1 = (1 < tmax) ? w2[ca.at(1)] : zero;
 #pragma unroll
       for (int t = 0; t < CP; t++) {
         const double2 x2 = (t + 2 < CP) ? ((t + 2 < tmax) ? w2[ca.at(t + 2 < CP ? t + 2 : 0)] : zero) : (t + 2 == CP ? hA : hB);
-        double2 b = zero;
-        const double2 l0 = ldg(cf[0] + t * TPL), l1 = ldg(cf[1] + t * TPL), l2 = ldg(cf[2] + t * TPL);
-        const double2 k0 = d2(fma(l0.x, wl[0], ad[0]), fma(l0.y, wl[0], ad[0]));
-        const double2 k1 = d2(fma(l1.x, wl[1], ad[1]), fma(l1.y, wl[1], ad[1]));
-        const double2 k2 = d2(fma(l2.x, wl[2], ad[2]), fma(l2.y, wl[2], ad[2]));
-        b = d2fma(k0, x0, d2fma(k1, x1, d2(k2.x * x2.x, k2.y * x2.y)));
+        double2 k0, k1, k2;
+        cf.at(2 * (p0 + t), k0, k1, k2);
+        double2 b = d2fma(k0, x0, d2fma(k1, x1, d2(k2.x * x2.x, k2.y * x2.y)));
         if (t >= tx) b.x = 0.0;
         if (t >= ty) b.y = 0.0;
         if (t < tmax) w2[ca.at(t)] = b;
@@ -510,7 +497,19 @@ __device__ __forceinline__ void fdma_fast_body(const LaneProg& P, const LaneOp& 
 }
 template <int E, int LN, int TPL>
 __device__ __noinline__ void fdma_fast(const LaneProg& P, const LaneOp& op, double* __restrict__ W, int gl, int lb, void* scratch) {
-  if (op.i2 & FD_PERLANE) fdma_fast_body<E, LN, TPL, true, false>(P, op, W, gl, lb, scratch);
-  else if (op.i2 & FD_PREBAND) fdma_fast_body<E, LN, TPL, false, true>(P, op, W, gl, lb, scratch);
-  else fdma_fast_body<E, LN, TPL, false, false>(P, op, W, gl, lb, scratch);
+  if (op.i2 & FD_PERLANE) { fdma_fast_body<E, LN, TPL, true, false>(P, op, W, gl, lb, scratch); return; }
+  if (op.i2 & FD_PREBAND) {
+    if constexpr (E <= 8) {   // Prog::band_solve folds the mat-vec on E <= 8 only: S^T of from_ortho, MatVecFdma of HholtzAdi
+      switch (band_terms((&op - 1)->i2)) {
+        case B2_BAND_TERMS(BC_UNIT, BC_S2_D, BC_ABSENT):
+          fdma_fast_body<E, LN, TPL, false, true, BandPairs<BC_UNIT, BC_S2_D, BC_ABSENT>>(P, op, W, gl, lb, scratch); break;
+        case B2_BAND_TERMS(BC_UNIT, BC_S2_N, BC_ABSENT):
+          fdma_fast_body<E, LN, TPL, false, true, BandPairs<BC_UNIT, BC_S2_N, BC_ABSENT>>(P, op, W, gl, lb, scratch); break;
+        case B2_BAND_TERMS(BC_PV0, BC_PV2, BC_PV4):
+          fdma_fast_body<E, LN, TPL, false, true, BandPairs<BC_PV0, BC_PV2, BC_PV4>>(P, op, W, gl, lb, scratch); break;
+      }
+    }
+    return;
+  }
+  fdma_fast_body<E, LN, TPL, false, false>(P, op, W, gl, lb, scratch);
 }

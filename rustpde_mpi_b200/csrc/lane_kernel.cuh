@@ -28,6 +28,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include "async_ops.cuh"
+#include "band_coef.cuh"
 
 #define B2_MAXOPS 24
 #define B2_MAXPEERS 8
@@ -38,10 +39,10 @@
 #define B2_PROGCOPY 2048 // shared-memory copy of the program header + ops (everything of LaneProg in front of tm[])
 
 enum LaneOpCode {
-  OP_LOAD = 1,     // W = [W +|*] a * src           i0=len  i2=flags(LD_*)       p0=src (p1 = stencil coefficients)
+  OP_LOAD = 1,     // W = [W +|*] a * src           i0=len  i2=flags(LD_*)       p0=src
   OP_STORE = 2,    // dst = [dst +] a * W            i0=len  i2=flags(ST_*)       p0=dst  (p1=peer table)
-  OP_BAND = 3,     // y_i = sum_m c_m[i] x_{i+o_m}   i0=len_out i1=packed offs i2=len_in  p0..p2 coef (null = 1, i1 byte=127: unused);
-                   //   generic geometry only (transform-sized lanes run OP_BANDC / OP_PREBAND)
+  OP_BAND = 3,     // y_i = sum_m c_m[i] x_{i+o_m}   i0=len_out i1=packed offs (byte=127: unused) i2=band_fams (term families and
+                   //   base size n, band_coef.cuh); generic geometry only (transform-sized lanes run OP_BANDC / OP_PREBAND)
   OP_DERIV = 4,    // Chebyshev d/dx of i0 coeffs, i1 times, times a
   OP_FDMA = 5,     // banded LU solve (fwd elim + back subst)  i0=len i2=flags(FD_*) p0=fl p1=inv_dia p2=u1 p3=u2 (fast geometry,
                    //   shared vectors: p0 = chunk-map table, LM_*)
@@ -62,12 +63,13 @@ enum LaneOpCode {
   OP_PDMA = 17,    // PdmaPlus2 solve (7 diagonals -2..+4, src/solver/pdma_plus2.rs:123-157): i0 = n, i1 = pitch L of the packed LU
                    //   p0 = [l2 shifted | ka | 1/mu | al | be | ga | de], each L doubles
 };
-enum { LD_ACC = 1, LD_PLAIN = 2, LD_MUL = 4, LD_STENCIL = 8,   // LD_STENCIL: value = src[j] + p1[j] * src[j-2]
+enum { LD_ACC = 1, LD_PLAIN = 2, LD_MUL = 4, LD_STENCIL = 8,   // LD_STENCIL: value = src[j] + s_{j-2} src[j-2], 2 <= j < len (= n)
        LD_TMA = 16,          // set by the launcher: the slab streams through the warps' staging slots (load_warps)
        LD_AFTER_STORE = 32,  // set by the launcher: the source was stored earlier in this program (flush stores first)
        LD_DIRECT = 64,       // set by the launcher: zero-copy TMA straight into W (plain load, a == 1)
        LD_PSPLIT = 128,      // plain sources: rows are stored parity-split (row r < i1 lives at r/2, odd rows after the even ones)
-       LD_PSPLITC = 256 };   // plain sources: the positions along the lane (columns) are stored parity-split, i1 = m0
+       LD_PSPLITC = 256,     // plain sources: the positions along the lane (columns) are stored parity-split, i1 = m0
+       LD_NEUMANN = 512 };   // LD_STENCIL of a ChebNeumann base (s_k = -(k/(k+2))^2); without it ChebDirichlet (s = -1)
 enum { ST_ACC = 1, ST_PLAIN = 2, ST_TRANS = 8, ST_PEER = 16,
        ST_TMA = 32,          // set by the launcher: staged, bulk tensor store / reduction
        ST_DIRECT = 64,       // set by the launcher: zero-copy TMA straight from W (same orientation, a == 1, no accumulate)
@@ -466,7 +468,7 @@ __device__ __noinline__ void load_warps(const LaneProg& P, const LaneOp& op, con
   const int w = threadIdx.x >> 5, ln = threadIdx.x & 31;
   const double a = op.a;
   const bool acc = op.i2 & LD_ACC, mul = op.i2 & LD_MUL, sten = op.i2 & LD_STENCIL;
-  const double* sc = reinterpret_cast<const double*>(op.p1);
+  const int sfam = (op.i2 & LD_NEUMANN) ? BC_STEN_N : BC_STEN_D;
   double2* W2 = reinterpret_cast<double2*>(sv.W);
   char* slot0 = sv.st + (size_t)w * 2 * P.wslot_bytes;
   uint64_t* bar = sv.wbar + 2 * w;
@@ -501,8 +503,8 @@ __device__ __noinline__ void load_warps(const LaneProg& P, const LaneOp& op, con
       double2 v = st[pc];
       if (sten && j0 >= 2) {
         const double2 u = (pc & 1) ? st[pc - 1] : st[pc - (1 << LSH) + 1];
-        const double2 cf = ldg(reinterpret_cast<const double2*>(sc + j0));
-        v.x = fma(cf.x, u.x, v.x); v.y = fma(cf.y, u.y, v.y);
+        const double cx = band_coef(sfam, j0, len), cy = band_coef(sfam, j0 + 1, len);
+        v.x = fma(cx, u.x, v.x); v.y = fma(cy, u.y, v.y);
       }
       v.x = (j0 < len) ? v.x * a : 0.0;
       v.y = (j0 + 1 < len) ? v.y * a : 0.0;
@@ -527,7 +529,7 @@ __device__ __noinline__ void load_threads(const LaneProg& P, const LaneOp& op, c
   const bool acc = op.i2 & LD_ACC, mul = op.i2 & LD_MUL, plain = op.i2 & LD_PLAIN, sten = op.i2 & LD_STENCIL;
   const double2* src = reinterpret_cast<const double2*>(op.p0);
   const size_t slab = (size_t)gl * P.in_tiles * 8;  // in double2 units
-  const double* sc = reinterpret_cast<const double*>(op.p1);
+  const int sfam = (op.i2 & LD_NEUMANN) ? BC_STEN_N : BC_STEN_D;
   double2* W2 = reinterpret_cast<double2*>(sv.W);
   const int psplit = (op.i2 & LD_PSPLIT) ? op.i1 : 0;   // rows < psplit of a plain source are stored parity-split
   if (op.i2 & LD_AFTER_STORE) wait_all_stores_complete();   // the source was written by this CTA's bulk stores
@@ -559,7 +561,7 @@ __device__ __noinline__ void load_threads(const LaneProg& P, const LaneOp& op, c
       if (pc >= npieces) break;
       const int j0 = 4 * (pc >> LSH) + (pc & 1) * 2;
       double2 x = v[k];
-      if (sten && j0 >= 2 && j0 < len) { x.x = fma(sc[j0], u[k].x, x.x); x.y = fma(sc[j0 + 1], u[k].y, x.y); }
+      if (sten && j0 >= 2 && j0 < len) { x.x = fma(band_coef(sfam, j0, len), u[k].x, x.x); x.y = fma(band_coef(sfam, j0 + 1, len), u[k].y, x.y); }
       x.x *= a;
       x.y = (j0 + 1 < len) ? x.y * a : 0.0;
       double2* w = W2 + pc;
@@ -791,28 +793,26 @@ __device__ __noinline__ void op_band(const LaneProg& P, const LaneOp& op, double
   const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
   const int len_out = op.i0;
   const int h0 = (int)(signed char)(op.i1 & 0xff), h1 = (int)(signed char)((op.i1 >> 8) & 0xff), h2 = (int)(signed char)((op.i1 >> 16) & 0xff);
-  const double2* __restrict__ c0 = (const double2*)op.p0;
-  const double2* __restrict__ c1 = (const double2*)op.p1;
-  const double2* __restrict__ c2 = (const double2*)op.p2;
+  const int n = band_n(op.i2);
   double2* w2 = reinterpret_cast<double2*>(W) + 2 * l;
   const double2 zero = d2(0.0, 0.0);
   double2 y[CP];
 #pragma unroll
   for (int t = 0; t < CP; t++) y[t] = zero;
-  auto term = [&](int h, const double2* __restrict__ c) {
+  auto term = [&](int h, int f) {
     const int hp = h >> 1;
 #pragma unroll
     for (int t = 0; t < CP; t++) {
       const int p = q + t * TPL, pp = p + hp;
       const bool ok = pp >= 0 && pp < HP && p < HP;
       const double2 x = w2[Lay<LN>::pix(ok ? pp : 0)];
-      const double2 cc = c ? ldg(c + (p < HP ? p : 0)) : d2(1.0, 1.0);
+      const double2 cc = d2(band_coef(f, 2 * p, n), band_coef(f, 2 * p + 1, n));
       if (ok) y[t] = d2fma(cc, x, y[t]);
     }
   };
-  if (h0 != 127) term(h0, c0);
-  if (h1 != 127) term(h1, c1);
-  if (h2 != 127) term(h2, c2);
+  if (h0 != 127) term(h0, band_fam(op.i2, 0));
+  if (h1 != 127) term(h1, band_fam(op.i2, 1));
+  if (h2 != 127) term(h2, band_fam(op.i2, 2));
   __syncthreads();
 #pragma unroll
   for (int t = 0; t < CP; t++) {
