@@ -100,6 +100,53 @@ def check_gradient(k0, n0, k1, n1, deriv, scale=(1.5, 1.0), seed=5):
     return relerr(fg.gradient(deriv, scale).get(), fo.gradient(deriv, scale))
 
 
+def op_errors(k0, n0, k1, n1, lane_axis):
+    """Every field operator of one space against the oracle: forward, backward, to_ortho, from_ortho, the gradients (1,0),
+    (0,1), (2,0), (0,2) and HholtzAdi (where neither axis is orthonormal Chebyshev) bounded by TOL; the third derivative along
+    ``lane_axis`` by max(TOL, 10 x yardstick), the rule of the other third-derivative checks.  Returns ({op: error}, {op:
+    (error, bound)} of the ops over their bound; NaN fails)."""
+    sp = (k0, n0, k1, n1)
+    errs = {op: globals()["check_" + op](*sp) for op in ("forward", "backward", "to_ortho", "from_ortho")}
+    errs.update({f"gradient{d}": check_gradient(*sp, d) for d in ((1, 0), (0, 1), (2, 0), (0, 2))})
+    if 0 not in (k0, k1):
+        errs["hholtz_adi"] = check_hholtz(*sp)
+    bound = {op: TOL for op in errs}
+    d3 = (3, 0) if lane_axis == 0 else (0, 3)
+    errs[f"gradient{d3}"], yard = check_gradient_yardstick(*sp, d3)
+    bound[f"gradient{d3}"] = max(TOL, 10.0 * yard)
+    return errs, {op: (e, bound[op]) for op, e in errs.items() if not e < bound[op]}
+
+
+def neumann_stencil_mismatches(k0, n0, k1, n1):
+    """to_ortho of a ChebNeumann lane next to an orthonormal Chebyshev axis (whose to_ortho is the identity), bit for bit.
+    Lane l holds vhat_k = 1 at k = l (mod 4) and 0 elsewhere, so that one lane group covers every residue; the stencil
+    ortho_j = vhat_j + s_{j-2} vhat_{j-2} then gives exactly 1 at j = l (mod 4), j < n - 2, exactly s_{j-2} = -((j-2) / j)^2
+    at j = l + 2 (mod 4) (Base1::init_host: the IEEE quotient, squared) and 0 elsewhere.  Returns (number of elements whose
+    bits differ, the first of them as (lane, j, got, want))."""
+    lane_axis = 1 if k1 == CN else 0
+    assert (k0, k1)[lane_axis] == CN and (k0, k1)[1 - lane_axis] == 0, (k0, k1)
+    n, lanes = (n0, n1)[lane_axis], (n0, n1)[1 - lane_axis]
+    m = n - 2
+    l = np.arange(lanes)[:, None]
+    k = np.arange(m)[None, :]
+    vhat = (k % 4 == l % 4).astype(np.float64)
+    j = np.arange(n)[None, :]
+    jm2 = np.maximum(j - 2, 0).astype(np.float64)
+    s = -(jm2 / (jm2 + 2.0)) ** 2
+    want = np.where((j % 4 == l % 4) & (j < m), 1.0, np.where((j % 4 == (l + 2) % 4) & (j >= 2), s, 0.0))
+    fg = b2.Field2(b2.Space2((k0, n0), (k1, n1)))
+    fg.vhat = vhat if lane_axis == 1 else vhat.T
+    got = fg.to_ortho().get()
+    if lane_axis == 0:
+        got = got.T
+    got, want = np.ascontiguousarray(got) + 0.0, want + 0.0   # + 0.0: -0 and +0 compare equal (s_0 = -0)
+    bad = np.argwhere(got.view(np.uint64) != want.view(np.uint64))
+    if len(bad) == 0:
+        return 0, None
+    li, ji = bad[0]
+    return len(bad), (int(li), int(ji), float(got[li, ji]), float(want[li, ji]))
+
+
 def perturbed(a, seed):
     """``a`` changed in the last bit: multiplied by 1 + 4e-16 N(0,1) (the conditioning yardstick's input)"""
     return a * (1.0 + 4e-16 * np.random.default_rng(seed).standard_normal(a.shape))
@@ -327,10 +374,21 @@ def navier_errors(no, ng):
     return out
 
 
-def check_navier(nx, ny, steps, periodic=False, ra=1e5, dt=0.01, init="modes", bc="rbc", mode=None):
+def share_tempbc(no, ng):
+    """Hand the oracle the CUDA side's boundary field tempbc.  Each side builds tempbc with its own grid, cos and transforms,
+    so the coefficients differ by a transform's round-off (~1e-15 of the largest); with bc = "hc" tempbc varies along x and the
+    step adds dt ka d2/dx2 tempbc, which multiplies that round-off in the high modes by ~k^4 (6e-10 in temp after two steps at
+    1025 x 129).  With the same tempbc on both sides the comparison measures the step alone."""
+    no.tempbc.vhat = np.array(ng.tempbc.vhat)
+    no.tempbc.backward()
+
+
+def check_navier(nx, ny, steps, periodic=False, ra=1e5, dt=0.01, init="modes", bc="rbc", mode=None, same_tempbc=False):
     """``mode``: the step schedule of the CUDA side (Navier2D.set_mode: bit 0 fused, bit 1 no CUDA-graph replay, bit 2 no
-    parallel branches); None keeps the default (fused, branches, graph replay)."""
+    parallel branches); None keeps the default (fused, branches, graph replay).  ``same_tempbc``: share_tempbc first."""
     no, ng = make_navier_pair(nx, ny, ra, 1.0, dt, 1.0, periodic, init, bc)
+    if same_tempbc:
+        share_tempbc(no, ng)
     if mode is not None:
         ng.set_mode(mode)
     for _ in range(steps):
@@ -339,11 +397,34 @@ def check_navier(nx, ny, steps, periodic=False, ra=1e5, dt=0.01, init="modes", b
     return navier_errors(no, ng)
 
 
-def check_navier_white_noise(nx, ny, steps, periodic=False, ra=1e5, dt=0.01):
+def check_navier_tempbc_yardstick(nx, ny, steps, ra=1e5, dt=0.01, bc="hc", seeds=(1, 2)):
+    """Smooth-state steps with each side's own tempbc: the errors of the CUDA path against the oracle AND the yardstick = the
+    largest change of the oracle when tempbc's coefficients get a transform's round-off, + 4e-16 max|vhat| N(0,1) on every
+    mode (share_tempbc: that round-off is the whole difference between the two sides' tempbc)."""
+    eig = b2.poisson_eig(b2.CHEB_NEUMANN, nx, 1.0)
+    ng = b2.Navier2D(nx, ny, ra, 1.0, dt, 1.0, bc)
+    navs = [ng] + [o.Navier2D(nx, ny, ra, 1.0, dt, 1.0, bc, pois_eig=eig) for _ in range(1 + len(seeds))]
+    for nav in navs:
+        nav.set_velocity(0.2, 1.0, 1.0)
+        nav.set_temperature(0.2, 1.0, 1.0)
+    no, refs = navs[1], navs[2:]
+    for nr, seed in zip(refs, seeds):
+        vh = nr.tempbc.vhat
+        nr.tempbc.vhat = vh + 4e-16 * np.abs(vh).max() * np.random.default_rng(seed).standard_normal(vh.shape)
+        nr.tempbc.backward()
+    for _ in range(steps):
+        for nav in [no] + refs:
+            nav.update()
+    ng.update(steps)
+    return navier_errors(no, ng), max(max(navier_errors(no, nr).values()) for nr in refs)
+
+
+def check_navier_white_noise(nx, ny, steps, periodic=False, ra=1e5, dt=0.01, bc="rbc", same_tempbc=False):
     """White-noise initial fields (U(-0.1, 0.1) in physical space, navier.rs:171-182).  The projection step cancels a large
     divergent part of the intermediate velocity, so the step itself is conditioned well above rounding: returns the errors of the
     CUDA path against the oracle AND the yardstick = the oracle against itself when the same input is changed in the last bit
-    (multiplied by 1 + 4e-16 N(0,1)); tests bound the error by max(TOL, 10 x yardstick) (same rule as test_gpu_parity_large)."""
+    (multiplied by 1 + 4e-16 N(0,1)); tests bound the error by max(TOL, 10 x yardstick) (same rule as test_gpu_parity_large).
+    ``same_tempbc``: both oracle runs take the CUDA side's tempbc (share_tempbc)."""
     def fields(perturb):
         out = {}
         for name, seed in (("temp", 1), ("velx", 2), ("vely", 3)):
@@ -360,14 +441,16 @@ def check_navier_white_noise(nx, ny, steps, periodic=False, ra=1e5, dt=0.01):
             fld.forward()
 
     eig = None if periodic else b2.poisson_eig(b2.CHEB_NEUMANN, nx, 1.0)
+    ng = b2.Navier2D(nx, ny, ra, 1.0, dt, 1.0, bc, periodic=periodic)
     refs = []
     for perturb in (False, True):
-        no = o.Navier2D(nx, ny, ra, 1.0, dt, 1.0, "rbc", periodic=periodic, pois_eig=eig)
+        no = o.Navier2D(nx, ny, ra, 1.0, dt, 1.0, bc, periodic=periodic, pois_eig=eig)
+        if same_tempbc:
+            share_tempbc(no, ng)
         start(no, perturb)
         for _ in range(steps):
             no.update()
         refs.append(no)
-    ng = b2.Navier2D(nx, ny, ra, 1.0, dt, 1.0, "rbc", periodic=periodic)
     start(ng, False)
     ng.update(steps)
     errs = navier_errors(refs[0], ng)

@@ -59,6 +59,16 @@ def test_instance_cdn_call_sequence(case, monkeypatch):
     assert_sequences(f"seq {case} {sid(sp)}", sp)
 
 
+CN_PLACED = [(c, sp, orient) for c, k, sp, orient in ti.KIND_PLACED if k == CN]
+
+
+@pytest.mark.parametrize("case,sp,orient", CN_PLACED, ids=[f"{c}-cn-axis{1 - o}" for c, _, o in CN_PLACED])
+def test_instance_cn_call_sequence(case, sp, orient, monkeypatch):
+    ti.set_env(monkeypatch, ti.CASE[case][1])
+    assert ti.layout_of(sp, orient) == ti.want(case)
+    assert_sequences(f"seq {case} {sid(sp)}", sp)
+
+
 @pytest.mark.parametrize("sp", [(R2C, 64, CDN, 65), (C2C, 16, CD, 65)], ids=sid)
 def test_call_sequence(sp, monkeypatch):
     ti.set_env(monkeypatch, {})
@@ -139,6 +149,16 @@ def test_navier_padding_in_every_schedule(mode, periodic, monkeypatch):
     ng.set_mode(mode)
     ng.update(3)
     assert_navier_padding(f"navier mode {mode} periodic {periodic}", ng)
+
+
+@pytest.mark.parametrize("mode", [1, 0, 3, 5], ids=["fused", "unfused", "fused-nograph", "fused-nobranches"])
+@pytest.mark.parametrize("periodic", [False, True])
+def test_navier_hc_padding_in_every_schedule(mode, periodic, monkeypatch):
+    ti.set_env(monkeypatch, {})
+    ng = g.b2.Navier2D(128 if periodic else 129, 129, 1e5, 1.0, 0.01, 1.0, "hc", periodic=periodic)
+    ng.set_mode(mode)
+    ng.update(3)
+    assert_navier_padding(f"navier hc mode {mode} periodic {periodic}", ng)
 
 
 @pytest.mark.parametrize("name", sorted(ti.STEPS))
