@@ -381,7 +381,8 @@ struct Base1 {
       }
   }
   int init_host(int kind_, int n_);
-  int init(int C, int TPL);   // device vectors; (C, TPL) = chunking of the passes whose lanes run along this axis
+  int init(int C, int TPL, bool fft);   // device vectors; (C, TPL) = chunking of the passes whose lanes run along this axis,
+                                        // fft = those passes have an FFT thread layout (PassCfg::fft)
   int lay_C = 1, lay_TPL = 1;
   void release() {
     tlu.release();
@@ -389,7 +390,14 @@ struct Base1 {
   }
 };
 
-static bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
+// Transform sizes the FFT core runs (N = n-1 for Chebyshev, n for r2c): N = f * 2^k >= 64 with f = 1, 3 or 5 (lane_fft: the
+// power-of-two passes, then one radix-f pass).  Returns f, or 0 for any other size.  Whether a size runs the FFT also needs a
+// thread layout (make_cfg, PassCfg::fft); sizes without one run the dense matrices up to 2049 points.
+static int fft_odd_factor(int N) {
+  if (N < 64) return 0;
+  const int P = N & -N, f = N / P;
+  return (f == 1 || f == 3 || f == 5) ? f : 0;
+}
 
 int Base1::init_host(int kind_, int n_) {
   kind = kind_; n = n_;
@@ -424,7 +432,7 @@ int Base1::init_host(int kind_, int n_) {
   return B2_OK;
 }
 
-int Base1::init(int C, int TPL) {
+int Base1::init(int C, int TPL, bool fft) {
   lay_C = C; lay_TPL = TPL;
   const int L = roundup(std::max(rows_phys, rows_ortho) + 8, 4) + 64;  // generous coefficient-vector length
   if (composite) {
@@ -451,8 +459,8 @@ int Base1::init(int C, int TPL) {
     pent_L = L;
     RET(d_pent.upload(pdma_sweep(m, d, L)));
   }
-  // transform tables (only when the size is one the FFT core handles)
-  if (is_pow2(N) && N >= 64) {
+  // transform tables (only when the size is one the FFT core handles and the lanes have an FFT thread layout)
+  if (fft) {
     const int M = N / 2;
     const long double PI = 3.14159265358979323846264338327950288L;
     std::vector<double> tw(2 * M), tw2(2 * (M + 1)), isin(M, 0.0);
@@ -504,7 +512,8 @@ int Base1::init(int C, int TPL) {
 
 struct PassCfg {
   int in_tiles, out_tiles, LP, TPL, C, E, groups, LN;
-  bool fast;   // transform-sized lane: N = 2*E*TPL and LP >= N + 4 (lane_fast.cuh)
+  bool fft;    // the lane runs the FFT core: E * TPL = N/2 (fft_odd_factor)
+  bool fast;   // transform-sized lane: N = 2^k = 2*E*TPL and LP >= N + 4 (lane_fast.cuh)
   int NT, CHW, nsc, wslot_bytes, CHD, nchd, w_off, st_off;   // copy-pipeline geometry (lane_kernel.cuh)
   size_t smem;
 };
@@ -928,11 +937,13 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
     const int Nc = N / 2;
     for (int e = want; e >= 4; e /= 2) {
       const int tpl = Nc / e;
-      if (tpl >= 8 && (tpl * LN) % 32 == 0 && tpl * LN <= 512 && tpl <= 256 && 2 * (e + 1) * tpl >= Pl) { c->E = e; c->TPL = tpl; c->LN = LN; return true; }
+      if (Nc % e == 0 && tpl >= 8 && (tpl * LN) % 32 == 0 && tpl * LN <= 512 && tpl <= 256 && 2 * (e + 1) * tpl >= Pl) { c->E = e; c->TPL = tpl; c->LN = LN; return true; }
     }
     return false;
   };
-  if (is_pow2(N) && N >= 64) {
+  const int f = fft_odd_factor(N);
+  c->fft = false;
+  if (f) {
     const int Nc = N / 2;
     int want = Nc >= 1024 ? 16 : (Nc >= 64 ? 8 : 4);   // short lanes: fewer points per thread = more threads per lane
     if (const char* e = getenv("B2_E")) {   // tuning knob
@@ -945,8 +956,10 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
     if (ln_want == 4 && smem4 <= 227 * 1024) ok = pick(4, want) || pick(4, 16);
     if (!ok) ok = pick(2, want) || pick(2, 16);
     if (!ok && smem4 <= 227 * 1024) ok = pick(4, want) || pick(4, 16);
-    if (!ok) return fail(B2_ERR_UNSUPPORTED, "lane of " + std::to_string(Pl) + " points: no supported thread layout");
-  } else {  // no transform along this axis: banded ops only
+    if (!ok && f == 1) return fail(B2_ERR_UNSUPPORTED, "lane of " + std::to_string(Pl) + " points: no supported thread layout");
+    c->fft = ok;   // 3 * 2^k, 5 * 2^k without a layout: dense transforms (up to 2049 points), as for any other size
+  }
+  if (!c->fft) {  // no FFT along this axis: banded ops only
     c->E = 16; c->LN = 4;
     int t = 8;
     while (2 * 17 * t < Pl) t *= 2;
@@ -955,7 +968,7 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
   }
   c->C = c->E + 1;
   c->NT = c->LN * c->TPL;
-  c->fast = is_pow2(N) && N >= 64 && N == 2 * c->E * c->TPL && Pl >= N + 4 && has_fast_instance(c->E, c->LN, c->TPL) && getenv("B2_NOFAST") == nullptr;
+  c->fast = c->fft && f == 1 && N == 2 * c->E * c->TPL && Pl >= N + 4 && has_fast_instance(c->E, c->LN, c->TPL) && getenv("B2_NOFAST") == nullptr;
   if (c->NT % 32) return fail(B2_ERR_UNSUPPORTED, "compute threads must fill whole warps");
   // shared memory: [mbarriers][program copy][scratch][W][per warp: 2 staging slots of CHW + 1 tiles]
   const int tile_bytes = c->LN * 32;
@@ -1025,7 +1038,7 @@ static bool shape_complex(const b2_space* sp, int shape_kind) { return !sp->b[0]
 // ------------------------------------------------------------------------------------------------
 static int op_forward(b2_space* sp, const double* v, double* vhat) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
-  if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64 runs the FFT core, other sizes up to 2049 a dense matrix; larger non-power-of-two sizes are not supported");
+  if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64, and 3 * 2^k or 5 * 2^k with a thread layout (193 / 192 points and up), runs the FFT core, other sizes up to 2049 a dense matrix; larger sizes of any other form are not supported");
   Prog y(sp, 0); y.load(v, b1.rows_phys); y.forward_ortho(b1); int l = y.from_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
   RET(run_pass(y));
   Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_phys); x.forward_ortho(b0); l = x.from_ortho(b0); x.store(vhat, l, ST_TRANS);
@@ -1033,7 +1046,7 @@ static int op_forward(b2_space* sp, const double* v, double* vhat) {
 }
 static int op_backward(b2_space* sp, const double* vhat, double* v) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
-  if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64 runs the FFT core, other sizes up to 2049 a dense matrix; larger non-power-of-two sizes are not supported");
+  if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64, and 3 * 2^k or 5 * 2^k with a thread layout (193 / 192 points and up), runs the FFT core, other sizes up to 2049 a dense matrix; larger sizes of any other form are not supported");
   Prog y(sp, 0); y.load(vhat, b1.rows_spec); y.to_ortho(b1); int l = y.backward_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
   RET(run_pass(y));
   Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); x.to_ortho(b0); l = x.backward_ortho(b0); x.store(v, l, ST_TRANS);
@@ -1573,8 +1586,8 @@ int b2_space2_create(b2_ctx* ctx, int kind0, int n0, int kind1, int n1, b2_space
   for (int ax = 0; ax < 2; ax++) sp->P[ax] = roundup(std::max(sp->b[ax].rows_phys, sp->b[ax].rows_ortho), 4 * ctx->nranks);
   r = make_cfg(sp->b[1], sp->P[1], sp->P[0], &sp->cfg[0], ctx->nranks);
   if (r == B2_OK) r = make_cfg(sp->b[0], sp->P[0], sp->P[1], &sp->cfg[1], ctx->nranks);
-  if (r == B2_OK) r = sp->b[1].init(sp->cfg[0].C, sp->cfg[0].TPL);   // cfg[0]: lanes along axis 1
-  if (r == B2_OK) r = sp->b[0].init(sp->cfg[1].C, sp->cfg[1].TPL);
+  if (r == B2_OK) r = sp->b[1].init(sp->cfg[0].C, sp->cfg[0].TPL, sp->cfg[0].fft);   // cfg[0]: lanes along axis 1
+  if (r == B2_OK) r = sp->b[0].init(sp->cfg[1].C, sp->cfg[1].TPL, sp->cfg[1].fft);
   if (r != B2_OK) { delete sp; return r; }
   sp->transforms_ok = (sp->b[0].d_tw.d || sp->b[0].dense_tr) && (sp->b[1].d_tw.d || sp->b[1].dense_tr);
   for (int i = 0; i < 3; i++) RET(alloc_zero(sp, &sp->tmp[i]));

@@ -226,11 +226,45 @@ template <> struct Dft<16> {
     }
   }
 };
+// odd radices (the last pass of an N = 3 * 2^k or 5 * 2^k plan): y_k = sum_j v_j w^{jk}, w = e^{-2 pi i / R}, written through
+// the conjugate-pair sums t = v_j + v_{R-j} and differences d = v_j - v_{R-j}
+template <> struct Dft<3> {
+  static __device__ __forceinline__ void run(cplx* v) {
+    const double s = 0.86602540378443864676;   // sin(2 pi/3)
+    const cplx t = cadd(v[1], v[2]), d = csub(v[1], v[2]);
+    const cplx m = make_double2(fma(-0.5, t.x, v[0].x), fma(-0.5, t.y, v[0].y));
+    v[0] = cadd(v[0], t);
+    v[1] = make_double2(fma(s, d.y, m.x), fma(-s, d.x, m.y));   // m - i s d
+    v[2] = make_double2(fma(-s, d.y, m.x), fma(s, d.x, m.y));   // m + i s d
+  }
+};
+template <> struct Dft<5> {
+  static __device__ __forceinline__ void run(cplx* v) {
+    const double c1 = 0.30901699437494742410, c2 = -0.80901699437494742410;   // cos(2 pi/5), cos(4 pi/5)
+    const double s1 = 0.95105651629515357212, s2 = 0.58778525229247312917;    // sin(2 pi/5), sin(4 pi/5)
+    const cplx t1 = cadd(v[1], v[4]), d1 = csub(v[1], v[4]), t2 = cadd(v[2], v[3]), d2 = csub(v[2], v[3]);
+    const cplx a = v[0];
+    const cplx m1 = make_double2(fma(c1, t1.x, fma(c2, t2.x, a.x)), fma(c1, t1.y, fma(c2, t2.y, a.y)));
+    const cplx m2 = make_double2(fma(c2, t1.x, fma(c1, t2.x, a.x)), fma(c2, t1.y, fma(c1, t2.y, a.y)));
+    const cplx n1 = make_double2(fma(s1, d1.x, s2 * d2.x), fma(s1, d1.y, s2 * d2.y));   // y_1 = m1 - i n1, y_4 = m1 + i n1
+    const cplx n2 = make_double2(fma(s2, d1.x, -s1 * d2.x), fma(s2, d1.y, -s1 * d2.y)); // y_2 = m2 - i n2, y_3 = m2 + i n2
+    v[0] = cadd(a, cadd(t1, t2));
+    v[1] = make_double2(m1.x + n1.y, m1.y - n1.x); v[4] = make_double2(m1.x - n1.y, m1.y + n1.x);
+    v[2] = make_double2(m2.x + n2.y, m2.y - n2.x); v[3] = make_double2(m2.x - n2.y, m2.y + n2.x);
+  }
+};
 
 // v[r] *= w1^r for r = 1..R-1.  The powers are generated in registers from the one loaded twiddle (chain
 // depth <= 4 multiplications, error a few ulp) instead of R-1 dependent table loads per butterfly.
 template <int R> struct Twid;
 template <> struct Twid<2> { static __device__ __forceinline__ void run(cplx* v, cplx w1) { v[1] = cmul(v[1], w1); } };
+template <> struct Twid<3> { static __device__ __forceinline__ void run(cplx* v, cplx w1) { v[1] = cmul(v[1], w1); v[2] = cmul(v[2], csq(w1)); } };
+template <> struct Twid<5> {
+  static __device__ __forceinline__ void run(cplx* v, cplx w1) {
+    const cplx w2 = csq(w1);
+    v[1] = cmul(v[1], w1); v[2] = cmul(v[2], w2); v[3] = cmul(v[3], cmul(w2, w1)); v[4] = cmul(v[4], csq(w2));
+  }
+};
 template <> struct Twid<4> {
   static __device__ __forceinline__ void run(cplx* v, cplx w1) {
     const cplx w2 = csq(w1);
@@ -949,16 +983,20 @@ __device__ __noinline__ void op_fdma(const LaneProg& P, const LaneOp& op, double
 // consecutive points (neighbouring q's write points of equal parity = the same bank pair): it writes point i at
 // i ^ ((i >> log2 E) & swz) and the following pass reads through the same map (swz = 1), which restores the
 // alternation; both sides are then conflict-free.
+// An odd radix R (3 or 5) runs only as the last pass, so Ns = Nc/R is still a power of two; E is not a multiple of R
+// there, so a thread runs ceil(E/R) butterflies and those past the Nc/R of the pass are skipped.
 template <int E, int R, bool FIRST, int LN>
 __device__ __forceinline__ void fft_stage(double2* __restrict__ wl, int Nc, int Ns, int q, int TPL, const cplx* __restrict__ tw,
                                           int swz_in, int swz_out) {
-  constexpr int NB = E / R, LE = Log2<E>::v;
-  cplx v[E];
+  constexpr int NB = (E + R - 1) / R, LE = Log2<E>::v;
+  constexpr bool PART = E % R != 0;
+  cplx v[NB * R];
   cplx w1[NB];
   const int stride = Nc / R;
 #pragma unroll
   for (int b = 0; b < NB; b++) {
     const int j = q + b * TPL;
+    if (PART && j >= stride) continue;
     if (!FIRST) w1[b] = ldg(tw + (j & (Ns - 1)) * (stride / Ns));   // issued ahead of the barrier
 #pragma unroll
     for (int r = 0; r < R; r++) {
@@ -971,6 +1009,7 @@ __device__ __forceinline__ void fft_stage(double2* __restrict__ wl, int Nc, int 
 #pragma unroll
   for (int b = 0; b < NB; b++) {
     const int j = q + b * TPL;
+    if (PART && j >= stride) continue;
     const int k = j & (Ns - 1);
     if (!FIRST) Twid<R>::run(v + b * R, w1[b]);
     Dft<R>::run(v + b * R);
@@ -985,19 +1024,31 @@ __device__ __forceinline__ void fft_stage(double2* __restrict__ wl, int Nc, int 
   __syncthreads();
 }
 
+// The odd pass as a call of its own: inlined, its ceil(E/R) * R points and ceil(E/R) twiddles per thread are allocated together
+// with the power-of-two passes and op_dct / op_rfft around them, and those spill (176 to 1564 bytes per op at E = 4 .. 16).
+template <int E, int R, int LN>
+__device__ __noinline__ void fft_stage_odd(double2* __restrict__ wl, int Nc, int q, int TPL, const cplx* __restrict__ tw, int swz_in) {
+  fft_stage<E, R, false, LN>(wl, Nc, Nc / R, q, TPL, tw, swz_in, 0);
+}
 template <int E, int LN>
 __device__ __forceinline__ void lane_fft(double* __restrict__ W, int Nc, int TPL, const cplx* __restrict__ tw) {
   const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
   double2* wl = reinterpret_cast<double2*>(W) + 2 * l;
-  // radix plan: as many radix-E passes as fit, then one pass with the remainder (1, 2, 4 or 8)
+  // radix plan for Nc = f * P, P = 2^j, f = 1, 3 or 5: as many radix-E passes over P as fit, then one pass with the
+  // remainder (1, 2, 4 or 8), then one radix-f pass
+  const int P = Nc & -Nc, f = Nc / P;
   int swz = (Nc > E) ? 1 : 0;
   fft_stage<E, E, true, LN>(wl, Nc, 1, q, TPL, tw, 0, swz);
   int Ns = E;
-  while (Nc / Ns >= E) { fft_stage<E, E, false, LN>(wl, Nc, Ns, q, TPL, tw, swz, 0); swz = 0; Ns *= E; }
-  const int rem = Nc / Ns;
+  while (P / Ns >= E) { fft_stage<E, E, false, LN>(wl, Nc, Ns, q, TPL, tw, swz, 0); swz = 0; Ns *= E; }
+  const int rem = P / Ns;
   if constexpr (E >= 16) { if (rem == 8) fft_stage<E, 8, false, LN>(wl, Nc, Ns, q, TPL, tw, swz, 0); }
   if constexpr (E >= 8) { if (rem == 4) fft_stage<E, 4, false, LN>(wl, Nc, Ns, q, TPL, tw, swz, 0); }
   if (rem == 2) fft_stage<E, 2, false, LN>(wl, Nc, Ns, q, TPL, tw, swz, 0);
+  if (f == 1) return;
+  if (rem > 1) swz = 0;   // the swizzled first pass has been read back; otherwise the odd pass is the second pass
+  if (f == 3) fft_stage_odd<E, 3, LN>(wl, Nc, q, TPL, tw, swz);
+  else fft_stage_odd<E, 5, LN>(wl, Nc, q, TPL, tw, swz);
 }
 
 // Chebyshev transform (DCT-I of n = N+1 points on Gauss-Lobatto nodes x_j = -cos(pi j/N)) through ONE
