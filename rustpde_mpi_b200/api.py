@@ -37,7 +37,8 @@ def fourier_r2c(n):
 
 
 def fourier_c2c(n):
-    """bases.rs:15: complex physical values, n modes in FFT order.  Not on the Navier2D path: dense-matrix transform, n <= 1024."""
+    """bases.rs:15: complex physical values, n modes in FFT order.  Not on the Navier2D path: axis 0 only, n <= 1024.  n = 2^k
+    (32 .. 1024) and 3 * 2^k, 5 * 2^k from 96 / 160 run the lane FFT; other n a dense-matrix transform."""
     return (FOURIER_C2C, n)
 
 

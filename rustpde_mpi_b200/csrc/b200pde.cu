@@ -327,7 +327,7 @@ struct Base1 {
   bool cdn = false;                        // ChebDirichletNeumann (bc = "hc"): three-term stencil, PdmaPlus2 solves
   bool c2c = false;                        // FourierC2c: complex physical values, n modes in FFT order (k = 0 .. n/2-1, -n/2 .. -1)
   int rows_phys = 0, rows_spec = 0, rows_ortho = 0;  // real rows along this axis (complex => 2 per mode)
-  int N = 0;                                          // transform size (n-1 Chebyshev, n Fourier)
+  int N = 0;                                          // transform size in reals (n-1 Chebyshev, n r2c, 2n c2c)
   std::vector<double> s2;                             // stencil: ortho_k = c_k + s2[k-2] c_{k-2} (the lane kernel forms it: band_coef.cuh)
   LuDev tlu;                                          // composite: from_ortho solve (S^T S) c = S^T o
   DVecD d_tw, d_tw2, d_isin;
@@ -390,8 +390,8 @@ struct Base1 {
   }
 };
 
-// Transform sizes the FFT core runs (N = n-1 for Chebyshev, n for r2c): N = f * 2^k >= 64 with f = 1, 3 or 5 (lane_fft: the
-// power-of-two passes, then one radix-f pass).  Returns f, or 0 for any other size.  Whether a size runs the FFT also needs a
+// Transform sizes the FFT core runs (N = n-1 for Chebyshev, n for r2c, 2n for c2c): N = f * 2^k >= 64 with f = 1, 3 or 5 (lane_fft:
+// the power-of-two passes, then one radix-f pass).  Returns f, or 0 for any other size.  Whether a size runs the FFT also needs a
 // thread layout (make_cfg, PassCfg::fft); sizes without one run the dense matrices up to 2049 points.
 static int fft_odd_factor(int N) {
   if (N < 64) return 0;
@@ -411,11 +411,11 @@ int Base1::init_host(int kind_, int n_) {
     m = (composite || cdn) ? n - 2 : n;
     rows_phys = n; rows_spec = m; rows_ortho = n; N = n - 1;
   } else if (c2c) {
-    // complex in, complex out (bases.rs:15): no Navier2D configuration uses it, so it runs the dense-matrix transform only
-    // (2n x 2n real matrix per lane, OP_DENSE) -- N = 0 keeps it off the FFT thread layouts
-    if (n > 1024) return fail(B2_ERR_UNSUPPORTED, "fourier_c2c: n <= 1024 (dense-matrix transform)");
+    // complex in, complex out (bases.rs:15): a lane of n complex points is N = 2n reals, laid out like an r2c lane of 2n points,
+    // so fft_odd_factor and make_cfg pick its FFT layout (OP_CFFT: an n-point complex FFT); other sizes run the dense matrices
+    if (n > 1024) return fail(B2_ERR_UNSUPPORTED, "fourier_c2c: n <= 1024");
     m = n;
-    rows_phys = 2 * n; rows_spec = 2 * n; rows_ortho = 2 * n; N = 0;
+    rows_phys = 2 * n; rows_spec = 2 * n; rows_ortho = 2 * n; N = 2 * n;
   } else {
     if (n % 2) return fail(B2_ERR_UNSUPPORTED, "fourier_r2c needs even n");
     m = n / 2 + 1;
@@ -465,6 +465,7 @@ int Base1::init(int C, int TPL, bool fft) {
     const long double PI = 3.14159265358979323846264338327950288L;
     std::vector<double> tw(2 * M), tw2(2 * (M + 1)), isin(M, 0.0);
     for (int t = 0; t < M; t++) { tw[2 * t] = (double)cosl(2 * PI * t / M); tw[2 * t + 1] = (double)(-sinl(2 * PI * t / M)); }
+    if (c2c) return d_tw.upload(tw);   // OP_CFFT is the M = n point FFT itself: no pre- / post-pass tables
     for (int j = 0; j <= M; j++) { tw2[2 * j] = (double)cosl(2 * PI * j / N); tw2[2 * j + 1] = (double)(-sinl(2 * PI * j / N)); }
     for (int k = 1; k < M; k++) isin[k] = (double)(1.0L / (4.0L * sinl(PI * k / N)));
     RET(d_tw.upload(tw)); RET(d_tw2.upload(tw2)); RET(d_isin.upload(isin));
@@ -513,7 +514,7 @@ int Base1::init(int C, int TPL, bool fft) {
 struct PassCfg {
   int in_tiles, out_tiles, LP, TPL, C, E, groups, LN;
   bool fft;    // the lane runs the FFT core: E * TPL = N/2 (fft_odd_factor)
-  bool fast;   // transform-sized lane: N = 2^k = 2*E*TPL and LP >= N + 4 (lane_fast.cuh)
+  bool fast;   // transform-sized lane: N = 2^k = 2*E*TPL and LP >= N + 4, or a c2c lane (lane_fast.cuh)
   int NT, CHW, nsc, wslot_bytes, CHD, nchd, w_off, st_off;   // copy-pipeline geometry (lane_kernel.cuh)
   size_t smem;
 };
@@ -710,6 +711,7 @@ struct Prog {
     LaneOp* o = add(OP_DCT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; o->p1 = b.d_tw2.d; o->p2 = b.d_isin.d; }
   void rfft(const Base1& b, int mode) {
     if (b.dense_tr) { if (mode == 0) dense(b.rows_ortho, b.rows_phys, b.d_dfwd.d); else dense(b.rows_phys, b.rows_ortho, b.d_dbwd.d); return; }
+    if (b.c2c) { LaneOp* o = add(OP_CFFT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; return; }
     LaneOp* o = add(OP_RFFT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; o->p1 = b.d_tw2.d; }
   void fdiff(int modes, int d, double scale, int wrap = 0) { LaneOp* o = add(OP_FDIFF); o->i0 = modes; o->i1 = d; o->a = scale; o->i2 = wrap; }
   void scalevec(int len, const double* v, int shift) { LaneOp* o = add(OP_SCALEVEC); o->i0 = len; o->i1 = shift; o->p0 = v; }
@@ -956,7 +958,9 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
     if (ln_want == 4 && smem4 <= 227 * 1024) ok = pick(4, want) || pick(4, 16);
     if (!ok) ok = pick(2, want) || pick(2, 16);
     if (!ok && smem4 <= 227 * 1024) ok = pick(4, want) || pick(4, 16);
-    if (!ok && f == 1) return fail(B2_ERR_UNSUPPORTED, "lane of " + std::to_string(Pl) + " points: no supported thread layout");
+    // Every c2c size has the dense transform (n <= 1024), so a c2c lane without a layout keeps it, e.g. n = 32 on 7 ranks (pitch 84
+    // against the 80 elements of E = 4, TPL = 8)
+    if (!ok && f == 1 && !lane_base.c2c) return fail(B2_ERR_UNSUPPORTED, "lane of " + std::to_string(Pl) + " points: no supported thread layout");
     c->fft = ok;   // 3 * 2^k, 5 * 2^k without a layout: dense transforms (up to 2049 points), as for any other size
   }
   if (!c->fft) {  // no FFT along this axis: banded ops only
@@ -968,7 +972,11 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
   }
   c->C = c->E + 1;
   c->NT = c->LN * c->TPL;
-  c->fast = c->fft && f == 1 && N == 2 * c->E * c->TPL && Pl >= N + 4 && has_fast_instance(c->E, c->LN, c->TPL) && getenv("B2_NOFAST") == nullptr;
+  // The fast ops of a Chebyshev / r2c lane reach past its N transform elements: the DCT writes element N, r2c's Nyquist pair
+  // sits at N, N + 1, and the band ops' chunks span 2 (E + 1) TPL elements.  A c2c lane has no padding (Pl = N = 2n): its only
+  // fast op, cfft_fast, touches elements 0 .. N - 1, and no banded op runs on a Fourier lane.
+  c->fast = c->fft && f == 1 && N == 2 * c->E * c->TPL && (Pl >= N + 4 || lane_base.c2c) && has_fast_instance(c->E, c->LN, c->TPL) &&
+            getenv("B2_NOFAST") == nullptr;
   if (c->NT % 32) return fail(B2_ERR_UNSUPPORTED, "compute threads must fill whole warps");
   // shared memory: [mbarriers][program copy][scratch][W][per warp: 2 staging slots of CHW + 1 tiles]
   const int tile_bytes = c->LN * 32;

@@ -218,6 +218,27 @@ __device__ __noinline__ void rfft_fast(const LaneProg& P, const LaneOp& op, doub
   }
 }
 
+// Complex FFT (see op_cfft), n = E*TPL points = the lane's 2n reals.
+template <int E, int LN, int TPL>
+__device__ __noinline__ void cfft_fast(const LaneOp& op, double* __restrict__ W) {
+  constexpr int PS = POff<LN, TPL>::v;
+  constexpr double s = 1.0 / (E * TPL);
+  const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
+  const cplx* tw = (const cplx*)op.p0;
+  cplx* w2 = reinterpret_cast<cplx*>(W) + 2 * l;
+  if (op.i1 == 0) { lane_fft_fast<E, LN, TPL>(W, l, q, tw); return; }
+  const int bk = Lay<LN>::pix(q);
+#pragma unroll
+  for (int i = 0; i < E; i++) w2[bk + i * PS] = cconj(w2[bk + i * PS]);
+  lane_fft_fast<E, LN, TPL>(W, l, q, tw);
+#pragma unroll
+  for (int i = 0; i < E; i++) {
+    const cplx z = w2[bk + i * PS];
+    w2[bk + i * PS] = make_double2(z.x * s, -z.y * s);
+  }
+  __syncthreads();
+}
+
 // ---------------------------------------------------------------------------------------------
 // chunked recurrences: thread q owns pairs p0 + t, p0 = q*CP, t < CP (CP = E + 1 odd).  pix(p0 + t) is
 // base_even + c(t) for even t and base_odd + c(t) for odd t with compile-time c: two runtime bases per thread.

@@ -62,6 +62,7 @@ enum LaneOpCode {
                    //   of sizes the FFT core does not handle (n - 1 / n not a power of two): O(n^2) per lane, small grids only
   OP_PDMA = 17,    // PdmaPlus2 solve (7 diagonals -2..+4, src/solver/pdma_plus2.rs:123-157): i0 = n, i1 = pitch L of the packed LU
                    //   p0 = [l2 shifted | ka | 1/mu | al | be | ga | de], each L doubles
+  OP_CFFT = 19,    // Fourier c2c, n complex points = the lane's 2n reals, modes in FFT order; i0 = n, i1: 0 fwd 1 bwd   p0=tw
 };
 enum { LD_ACC = 1, LD_PLAIN = 2, LD_MUL = 4, LD_STENCIL = 8,   // LD_STENCIL: value = src[j] + s_{j-2} src[j-2], 2 <= j < len (= n)
        LD_TMA = 16,          // set by the launcher: the slab streams through the warps' staging slots (load_warps)
@@ -1167,6 +1168,27 @@ __device__ __noinline__ void op_rfft(const LaneProg& P, const LaneOp& op, double
   }
 }
 
+// Complex FFT of n points along the lane (FourierC2c): pair k of the lane is point k (physical) or mode k (spectral, natural FFT
+// order).  Forward is unnormalised; backward is conj -> FFT -> conj with 1/n.  Nothing past element 2n - 1 is written.
+// The conjugation needs no barrier before the FFT: its first pass reads exactly the points q + r TPL that thread q conjugated.
+template <int E, int LN>
+__device__ __noinline__ void op_cfft(const LaneProg& P, const LaneOp& op, double* __restrict__ W) {
+  const int TPL = P.TPL;
+  const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
+  const int n = op.i0;
+  const cplx* tw = (const cplx*)op.p0;
+  cplx* w2 = reinterpret_cast<cplx*>(W) + 2 * l;
+  if (op.i1 == 0) { lane_fft<E, LN>(W, n, TPL, tw); return; }
+  for (int k = q; k < n; k += TPL) w2[Lay<LN>::pix(k)] = cconj(w2[Lay<LN>::pix(k)]);
+  lane_fft<E, LN>(W, n, TPL, tw);
+  const double s = 1.0 / n;
+  for (int k = q; k < n; k += TPL) {
+    const cplx z = w2[Lay<LN>::pix(k)];
+    w2[Lay<LN>::pix(k)] = make_double2(z.x * s, -z.y * s);
+  }
+  __syncthreads();
+}
+
 // ChebDirichletNeumann stencil (bc = "hc"): the three-term stencil couples neighbouring elements, so the pair structure of
 // the other banded operators does not apply; element-strided, register-staged (not on any BASELINE configuration's path).
 template <int CP, int LN>
@@ -1377,6 +1399,9 @@ __global__ void B2_LB lane_kernel(const __grid_constant__ LaneProg Pp) {
         break;
       case OP_RFFT:
         if constexpr (TPLC > 0) rfft_fast<E, LN, TPLC>(P, op, W); else op_rfft<E, LN>(P, op, W);
+        break;
+      case OP_CFFT:
+        if constexpr (TPLC > 0) cfft_fast<E, LN, TPLC>(op, W); else op_cfft<E, LN>(P, op, W);
         break;
       case OP_PREBAND: break;
       case OP_BANDC:
