@@ -35,7 +35,7 @@ enum b2_base_kind {
   B2_CHEB_NEUMANN = 2,
   B2_CHEB_DIRICHLET_NEUMANN = 3, /* bc="hc": three-term stencil, PdmaPlus2 solves (src/solver/pdma_plus2.rs) */
   B2_FOURIER_R2C = 4,
-  B2_FOURIER_C2C = 5 /* not on the Navier2D path: axis 0 only, n <= 1024, complex physical values; n = 2^k, 3 * 2^k, 5 * 2^k >= 32 with a thread layout run the lane FFT, other n a dense matrix */
+  B2_FOURIER_C2C = 5 /* not on the Navier2D path: axis 0 only.  Next to a Chebyshev axis 1: n <= 1024, complex physical values; n = 2^k, 3 * 2^k, 5 * 2^k >= 32 with a thread layout run the lane FFT, other n a dense matrix.  Next to FOURIER_R2C (doubly periodic): even n, real physical values (nx, ny), spectrum complex (nx, ny/2 + 1) row-major, x modes in FFT order; sizes as for r2c */
 };
 enum b2_shape_kind { B2_SHAPE_PHYSICAL = 0, B2_SHAPE_SPECTRAL = 1, B2_SHAPE_ORTHO = 2 };
 enum b2_status { B2_OK = 0, B2_ERR_ARG = 1, B2_ERR_CUDA = 2, B2_ERR_UNSUPPORTED = 3, B2_ERR_SHAPE = 4 };

@@ -37,8 +37,10 @@ def fourier_r2c(n):
 
 
 def fourier_c2c(n):
-    """bases.rs:15: complex physical values, n modes in FFT order.  Not on the Navier2D path: axis 0 only, n <= 1024.  n = 2^k
-    (32 .. 1024) and 3 * 2^k, 5 * 2^k from 96 / 160 run the lane FFT; other n a dense-matrix transform."""
+    """bases.rs:15: n modes in FFT order.  Not on the Navier2D path: axis 0 only.  Next to a Chebyshev axis 1: complex physical
+    values, n <= 1024; n = 2^k (32 .. 1024) and 3 * 2^k, 5 * 2^k from 96 / 160 run the lane FFT, other n a dense-matrix transform.
+    Next to ``fourier_r2c`` (a doubly periodic space, examples/swift_hohenberg_2d.rs): even n, real physical values, spectrum
+    complex (n, ny/2 + 1) = numpy's ``rfft2``; the sizes of an r2c axis (lane FFT up to 8192, dense matrices up to 2049)."""
     return (FOURIER_C2C, n)
 
 

@@ -326,8 +326,13 @@ struct Base1 {
   bool cheb = false, composite = false;   // composite: ChebDirichlet / ChebNeumann (stencil at even offsets: pair-structured lane operators)
   bool cdn = false;                        // ChebDirichletNeumann (bc = "hc"): three-term stencil, PdmaPlus2 solves
   bool c2c = false;                        // FourierC2c: complex physical values, n modes in FFT order (k = 0 .. n/2-1, -n/2 .. -1)
+  bool split = false;                      // FourierC2c axis 0 next to a FourierR2c axis 1 (doubly periodic): real physical values,
+                                           //   and the (Re, Im) pairs run along axis 1, so this axis holds one real per mode and its
+                                           //   lanes are split c2c lanes (lane_kernel.cuh, op_split): an r2c lane of n points plus OP_CPAIR
   int rows_phys = 0, rows_spec = 0, rows_ortho = 0;  // real rows along this axis (complex => 2 per mode)
-  int N = 0;                                          // transform size in reals (n-1 Chebyshev, n r2c, 2n c2c)
+  int N = 0;                                          // transform size in reals (n-1 Chebyshev, n r2c and split c2c, 2n c2c)
+  bool c2c_lane() const { return c2c && !split; }    // the lane holds n complex points (OP_CFFT)
+  int lane_rows() const { return split ? n + 2 : std::max(rows_phys, rows_ortho); }   // split: the half spectra of OP_RFFT
   std::vector<double> s2;                             // stencil: ortho_k = c_k + s2[k-2] c_{k-2} (the lane kernel forms it: band_coef.cuh)
   LuDev tlu;                                          // composite: from_ortho solve (S^T S) c = S^T o
   DVecD d_tw, d_tw2, d_isin;
@@ -380,7 +385,7 @@ struct Base1 {
         d[off + 2][off >= 0 ? i : j] = v;
       }
   }
-  int init_host(int kind_, int n_);
+  int init_host(int kind_, int n_, bool split_ = false);
   int init(int C, int TPL, bool fft);   // device vectors; (C, TPL) = chunking of the passes whose lanes run along this axis,
                                         // fft = those passes have an FFT thread layout (PassCfg::fft)
   int lay_C = 1, lay_TPL = 1;
@@ -399,17 +404,24 @@ static int fft_odd_factor(int N) {
   return (f == 1 || f == 3 || f == 5) ? f : 0;
 }
 
-int Base1::init_host(int kind_, int n_) {
+int Base1::init_host(int kind_, int n_, bool split_) {
   kind = kind_; n = n_;
   cheb = (kind <= B2_CHEB_DIRICHLET_NEUMANN);
   composite = (kind == B2_CHEB_DIRICHLET || kind == B2_CHEB_NEUMANN);
   cdn = (kind == B2_CHEB_DIRICHLET_NEUMANN);
   c2c = (kind == B2_FOURIER_C2C);
+  split = c2c && split_;
   if (kind < 0 || kind > B2_FOURIER_C2C) return fail(B2_ERR_ARG, "bad base kind");
   if (n < 5) return fail(B2_ERR_ARG, "n too small");
   if (cheb) {
     m = (composite || cdn) ? n - 2 : n;
     rows_phys = n; rows_spec = m; rows_ortho = n; N = n - 1;
+  } else if (split) {
+    // doubly periodic: the lanes are real sequences of n points (OP_RFFT, or the r2c dense matrices) whose half spectra OP_CPAIR
+    // combines in pairs of lanes, so sizes and layouts follow the r2c rules; the spectrum has one real row per mode
+    if (n % 2) return fail(B2_ERR_UNSUPPORTED, "fourier_c2c next to fourier_r2c needs even n");
+    m = n;
+    rows_phys = n; rows_spec = n; rows_ortho = n; N = n;
   } else if (c2c) {
     // complex in, complex out (bases.rs:15): a lane of n complex points is N = 2n reals, laid out like an r2c lane of 2n points,
     // so fft_odd_factor and make_cfg pick its FFT layout (OP_CFFT: an n-point complex FFT); other sizes run the dense matrices
@@ -465,7 +477,7 @@ int Base1::init(int C, int TPL, bool fft) {
     const long double PI = 3.14159265358979323846264338327950288L;
     std::vector<double> tw(2 * M), tw2(2 * (M + 1)), isin(M, 0.0);
     for (int t = 0; t < M; t++) { tw[2 * t] = (double)cosl(2 * PI * t / M); tw[2 * t + 1] = (double)(-sinl(2 * PI * t / M)); }
-    if (c2c) return d_tw.upload(tw);   // OP_CFFT is the M = n point FFT itself: no pre- / post-pass tables
+    if (c2c_lane()) return d_tw.upload(tw);   // OP_CFFT is the M = n point FFT itself: no pre- / post-pass tables
     for (int j = 0; j <= M; j++) { tw2[2 * j] = (double)cosl(2 * PI * j / N); tw2[2 * j + 1] = (double)(-sinl(2 * PI * j / N)); }
     for (int k = 1; k < M; k++) isin[k] = (double)(1.0L / (4.0L * sinl(PI * k / N)));
     RET(d_tw.upload(tw)); RET(d_tw2.upload(tw2)); RET(d_isin.upload(isin));
@@ -473,7 +485,7 @@ int Base1::init(int C, int TPL, bool fft) {
     // any other size: the transforms as dense matrices (SURVEY A.1 / A.4), applied per lane by OP_DENSE -- O(n^2) per lane, meant
     // for small grids such as the reference's criterion sizes (128, 264, 265, 512)
     const long double PI = 3.14159265358979323846264338327950288L;
-    if (c2c) {    // c_k = sum_j v_j e^{-2 pi i j k / n} (unnormalised), v_j = 1/n sum_k c_k e^{+2 pi i j k / n}; rows 2k, 2k+1 = Re, Im
+    if (c2c_lane()) {    // c_k = sum_j v_j e^{-2 pi i j k / n} (unnormalised), v_j = 1/n sum_k c_k e^{+2 pi i j k / n}; rows 2k, 2k+1 = Re, Im
       std::vector<double> F((size_t)4 * n * n), B((size_t)4 * n * n);
       const size_t w = (size_t)2 * n;
       for (int k = 0; k < n; k++)
@@ -496,7 +508,8 @@ int Base1::init(int C, int TPL, bool fft) {
           B[(size_t)j * n + k] = (double)(sg * c);
         }
       RET(d_dfwd.upload(F)); RET(d_dbwd.upload(B));
-    } else {      // r2c (unnormalised) / c2r (1/n): rows 2k, 2k+1 = Re, Im of mode k
+    } else {      // r2c (unnormalised) / c2r (1/n): rows 2k, 2k+1 = Re, Im of mode k (also the lanes of a split c2c axis)
+      const int m = n / 2 + 1;
       std::vector<double> F((size_t)2 * m * n), B((size_t)n * 2 * m);
       for (int k = 0; k < m; k++)
         for (int j = 0; j < n; j++) {
@@ -552,6 +565,7 @@ struct GemmPlan {
 struct b2_solver {
   b2_space* sp = nullptr;
   int type = 0;  // 0 hholtz_adi, 1 poisson
+  bool diag2 = false;   // poisson / hholtz with both axes Fourier: sd[0] = lam0 + alpha per x mode, sd[1] = mu1 per y real column
   // per axis: banded LU (Chebyshev) or reciprocal diagonal (Fourier)
   LuDev lu[2];
   DVecD sd[2], pd[2];   // pd: packed PdmaPlus2 LU (ChebDirichletNeumann axis)
@@ -709,11 +723,23 @@ struct Prog {
   void dct(const Base1& b, int mode) {
     if (b.dense_tr) { dense(b.n, b.n, mode == 0 ? b.d_dfwd.d : b.d_dbwd.d); return; }
     LaneOp* o = add(OP_DCT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; o->p1 = b.d_tw2.d; o->p2 = b.d_isin.d; }
+  // split c2c axis: the real transform of each lane, then OP_CPAIR (backward: OP_CPAIR first)
   void rfft(const Base1& b, int mode) {
-    if (b.dense_tr) { if (mode == 0) dense(b.rows_ortho, b.rows_phys, b.d_dfwd.d); else dense(b.rows_phys, b.rows_ortho, b.d_dbwd.d); return; }
-    if (b.c2c) { LaneOp* o = add(OP_CFFT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; return; }
-    LaneOp* o = add(OP_RFFT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; o->p1 = b.d_tw2.d; }
+    if (b.split && mode == 1) cpair(b.n, 1);
+    const int half = b.split ? b.n + 2 : b.rows_ortho;   // reals of the lane's half spectrum
+    if (b.dense_tr) {
+      if (mode == 0) dense(half, b.rows_phys, b.d_dfwd.d); else dense(b.rows_phys, half, b.d_dbwd.d);
+    } else if (b.c2c_lane()) {
+      LaneOp* o = add(OP_CFFT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d;
+    } else {
+      LaneOp* o = add(OP_RFFT); o->i0 = b.n; o->i1 = mode; o->p0 = b.d_tw.d; o->p1 = b.d_tw2.d;
+    }
+    if (b.split && mode == 0) cpair(b.n, 0);
+  }
+  void cpair(int n, int mode) { LaneOp* o = add(OP_CPAIR); o->i0 = n; o->i1 = mode; }
   void fdiff(int modes, int d, double scale, int wrap = 0) { LaneOp* o = add(OP_FDIFF); o->i0 = modes; o->i1 = d; o->a = scale; o->i2 = wrap; }
+  void sdiff(int n, int d, double scale) { LaneOp* o = add(OP_SDIFF); o->i0 = n; o->i1 = d; o->a = scale; }
+  void diag2(int n, int lanes, const double* lam, const double* mu) { LaneOp* o = add(OP_DIAG2); o->i0 = n; o->i1 = lanes; o->p0 = lam; o->p1 = mu; }
   void scalevec(int len, const double* v, int shift) { LaneOp* o = add(OP_SCALEVEC); o->i0 = len; o->i1 = shift; o->p0 = v; }
   void zerotail(int from) { LaneOp* o = add(OP_ZEROTAIL); o->i0 = from; }
   void lanemask(int from) { LaneOp* o = add(OP_LANEMASK); o->i0 = from; }
@@ -747,7 +773,7 @@ struct Prog {
   }
   int deriv_axis(const Base1& b, int d, double sc) {  // on ortho coefficients; sc = 1/scale^d
     if (d == 0) { if (sc != 1.0) scale(sc); return b.rows_ortho; }
-    if (b.cheb) deriv(b.n, d, sc); else fdiff(b.m, d, sc, b.c2c ? b.n : 0);
+    if (b.cheb) deriv(b.n, d, sc); else if (b.split) sdiff(b.n, d, sc); else fdiff(b.m, d, sc, b.c2c ? b.n : 0);
     return b.rows_ortho;
   }
   int backward_ortho(const Base1& b) {  // ortho coefficients -> physical values
@@ -960,7 +986,7 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
     if (!ok && smem4 <= 227 * 1024) ok = pick(4, want) || pick(4, 16);
     // Every c2c size has the dense transform (n <= 1024), so a c2c lane without a layout keeps it, e.g. n = 32 on 7 ranks (pitch 84
     // against the 80 elements of E = 4, TPL = 8)
-    if (!ok && f == 1 && !lane_base.c2c) return fail(B2_ERR_UNSUPPORTED, "lane of " + std::to_string(Pl) + " points: no supported thread layout");
+    if (!ok && f == 1 && !lane_base.c2c_lane()) return fail(B2_ERR_UNSUPPORTED, "lane of " + std::to_string(Pl) + " points: no supported thread layout");
     c->fft = ok;   // 3 * 2^k, 5 * 2^k without a layout: dense transforms (up to 2049 points), as for any other size
   }
   if (!c->fft) {  // no FFT along this axis: banded ops only
@@ -975,7 +1001,7 @@ static int make_cfg(const Base1& lane_base, int Pl, int Pc, PassCfg* c, int nran
   // The fast ops of a Chebyshev / r2c lane reach past its N transform elements: the DCT writes element N, r2c's Nyquist pair
   // sits at N, N + 1, and the band ops' chunks span 2 (E + 1) TPL elements.  A c2c lane has no padding (Pl = N = 2n): its only
   // fast op, cfft_fast, touches elements 0 .. N - 1, and no banded op runs on a Fourier lane.
-  c->fast = c->fft && f == 1 && N == 2 * c->E * c->TPL && (Pl >= N + 4 || lane_base.c2c) && has_fast_instance(c->E, c->LN, c->TPL) &&
+  c->fast = c->fft && f == 1 && N == 2 * c->E * c->TPL && (Pl >= N + 4 || lane_base.c2c_lane()) && has_fast_instance(c->E, c->LN, c->TPL) &&
             getenv("B2_NOFAST") == nullptr;
   if (c->NT % 32) return fail(B2_ERR_UNSUPPORTED, "compute threads must fill whole warps");
   // shared memory: [mbarriers][program copy][scratch][W][per warp: 2 staging slots of CHW + 1 tiles]
@@ -1039,7 +1065,15 @@ static int shape_of(const b2_space* sp, int shape_kind, int* rows, int* cols) {
   }
   return fail(B2_ERR_ARG, "bad shape kind");
 }
-static bool shape_complex(const b2_space* sp, int shape_kind) { return !sp->b[0].cheb && (shape_kind != B2_SHAPE_PHYSICAL || sp->b[0].c2c); }
+// The axis along which a complex array keeps its (Re, Im) pairs, or -1 for a real array.  0: rows 2k, 2k + 1 of axis 0 (a Fourier
+// axis 0 next to a Chebyshev axis 1; the host sees them interleaved, k_host_layout).  1: columns 2k, 2k + 1 of axis 1 (the spectrum
+// of a doubly periodic space, a row-major complex array as it is on the host; its physical values are real).
+static int pair_axis(const b2_space* sp, int shape_kind) {
+  const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
+  if (!b1.cheb) return shape_kind == B2_SHAPE_PHYSICAL ? -1 : 1;
+  return (!b0.cheb && (shape_kind != B2_SHAPE_PHYSICAL || b0.c2c)) ? 0 : -1;
+}
+static bool shape_complex(const b2_space* sp, int shape_kind) { return pair_axis(sp, shape_kind) >= 0; }
 
 // ------------------------------------------------------------------------------------------------
 // field operators (2 passes each: along y, transpose, along x, transpose back)
@@ -1055,6 +1089,16 @@ static int op_forward(b2_space* sp, const double* v, double* vhat) {
 static int op_backward(b2_space* sp, const double* vhat, double* v) {
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "transform size: n-1 (Chebyshev) / n (Fourier) = 2^k >= 64, and 3 * 2^k or 5 * 2^k with a thread layout (193 / 192 points and up), runs the FFT core, other sizes up to 2049 a dense matrix; larger sizes of any other form are not supported");
+  if (b0.split) {
+    // doubly periodic: the inverse along x comes first (the c2r along y needs every x of a mode, and mode kx pairs with row
+    // n - kx, which another CTA holds), so a transpose-only pass brings vhat into the x-lane orientation
+    Prog t(sp, 0); t.load(vhat, b1.rows_spec); t.store(sp->tmp[0], b1.rows_spec, ST_TRANS);
+    RET(run_pass(t));
+    Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); int l = x.backward_ortho(b0); x.store(sp->tmp[1], l, ST_TRANS);
+    RET(run_pass(x));
+    Prog y(sp, 0); y.load(sp->tmp[1], b1.rows_ortho); l = y.backward_ortho(b1); y.store(v, l, 0);
+    return run_pass(y);
+  }
   Prog y(sp, 0); y.load(vhat, b1.rows_spec); y.to_ortho(b1); int l = y.backward_ortho(b1); y.store(sp->tmp[0], l, ST_TRANS);
   RET(run_pass(y));
   Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_spec); x.to_ortho(b0); l = x.backward_ortho(b0); x.store(v, l, ST_TRANS);
@@ -1130,7 +1174,7 @@ static int hholtz_create(b2_space* sp, double c0, double c1, b2_solver** out) {
       b.cdn_hholtz_diags(c[ax], d);
       s->pd_L[ax] = L;
       RET(s->pd[ax].upload(pdma_sweep(b.m, d, L)));
-    } else if (!b.cheb) {  // Sdma: dia = 1 - c * (-k^2), src/solver/sdma.rs:37-46
+    } else if (!b.cheb) {  // Sdma: dia = 1 - c * (-k^2), src/solver/sdma.rs:37-46 (one entry per mode: emit_hh_axis)
       std::vector<double> sd(L, 0.0);
       for (int k = 0; k < b.m; k++) {
         const double kk = (b.c2c && 2 * k >= b.n) ? k - b.n : k;   // FourierC2c: modes in FFT order
@@ -1248,6 +1292,25 @@ static int poisson_create(b2_space* sp, double c0, double c1, const double* lam_
   const double alpha = hholtz ? 1.0 : 0.0;
   if (hholtz) { c0 = -c0; c1 = -c1; }
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
+  if (b0.split) {
+    // both axes Fourier: FdmaTensor's lane systems (lap1 + (lam_i + alpha) mass1) are diagonal, so the solve is one division per
+    // mode by (lam0[kx] + alpha) + mu1[ky], lam0 = -c0 kx^2 (FFT order) with the singularity shift of poisson.rs:84-86 on the whole
+    // vector, mu1 = -c1 ky^2 (OP_DIAG2 along x: element kx of lane 2 ky + r)
+    b2_solver* s = new b2_solver();
+    s->sp = sp; s->type = 1; s->diag2 = true;
+    std::vector<double> lam(b0.m), mu(b1.rows_spec);
+    for (int k = 0; k < b0.m; k++) {
+      const double kk = 2 * k >= b0.n ? k - b0.n : k;
+      lam[k] = -kk * kk * c0;
+    }
+    if (!hholtz && std::fabs(lam[0]) < 1e-10) for (auto& v : lam) v -= 1e-10;
+    for (auto& v : lam) v += alpha;
+    for (int k = 0; k < b1.m; k++) mu[2 * k] = mu[2 * k + 1] = -(double)k * k * c1;
+    const int r1 = s->sd[0].upload(lam), r2 = r1 == B2_OK ? s->sd[1].upload(mu) : r1;
+    if (r2 != B2_OK) { b2_solver_destroy(s); return r2; }
+    *out = s;
+    return B2_OK;
+  }
   if (!b1.composite) return fail(B2_ERR_UNSUPPORTED, "Poisson needs a composite Chebyshev axis 1");
   b2_solver* s = new b2_solver();
   s->sp = sp; s->type = 1;
@@ -1378,6 +1441,14 @@ static int poisson_solve(b2_solver* s, const double* in, double* out, bool zero0
   b2_ctx* ctx = sp->ctx;
   const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
   const int P0 = sp->P[0], P1 = sp->P[1];
+  if (s->diag2) {
+    Prog y(sp, 0); y.load(in, b1.rows_ortho); y.store(sp->tmp[0], b1.rows_spec, ST_TRANS);
+    RET(run_pass(y));
+    Prog x(sp, 1); x.load(sp->tmp[0], b0.rows_ortho); x.diag2(b0.m, b1.rows_spec, s->sd[0].d, s->sd[1].d);
+    if (zero00) { x.zeroelem(0, 0); x.zeroelem(1, 0); }   // Re and Im of mode (0, 0): lanes 0, 1 (pairs along axis 1)
+    x.store(out, b0.rows_spec, ST_TRANS);
+    return run_pass(x);
+  }
   if (s->dense) {
     // matvec along y and x (two transposing passes: back in the y-lane orientation, rows = x index), then the core
     Prog y(sp, 0); y.load(in, b1.rows_ortho); int l = y.matvec(b1); y.store(sp->tmp[0], l, ST_TRANS);
@@ -1402,7 +1473,7 @@ static void emit_hh_axis(Prog& p, const b2_solver* s, int ax) {
   if (b.composite) { p.band_solve(b.m, b.n, BC_PV0, BC_PV2, BC_PV4, s->lu[ax]); return; }
   p.matvec(b);
   if (b.cdn) p.pdma(b.m, s->pd[ax].d, s->pd_L[ax]);   // hholtz_adi.rs:64
-  else p.scalevec(b.rows_spec, s->sd[ax].d, 1);
+  else p.scalevec(b.rows_spec, s->sd[ax].d, b.split ? 0 : 1);   // a split c2c lane holds one real per mode
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1586,12 +1657,15 @@ int b2_space2_create(b2_ctx* ctx, int kind0, int n0, int kind1, int n1, b2_space
   CK(cudaSetDevice(ctx->device));
   b2_space* sp = new b2_space();
   sp->ctx = ctx;
-  int r = sp->b[0].init_host(kind0, n0);
+  // fourier_c2c x fourier_r2c (doubly periodic) runs its axis 0 as split c2c lanes
+  const bool dp = kind0 == B2_FOURIER_C2C && kind1 == B2_FOURIER_R2C;
+  int r = sp->b[0].init_host(kind0, n0, dp);
   if (r == B2_OK) r = sp->b[1].init_host(kind1, n1);
-  if (r == B2_OK && !sp->b[1].cheb) r = fail(B2_ERR_UNSUPPORTED, "axis 1 must be a Chebyshev base (Navier2D spaces)");
+  if (r == B2_OK && !sp->b[1].cheb && !dp)
+    r = fail(B2_ERR_UNSUPPORTED, "axis 1 must be a Chebyshev base, or fourier_r2c next to a fourier_c2c axis 0 (doubly periodic)");
   if (r != B2_OK) { delete sp; return r; }
   // padded so that the 4-row lane groups split evenly over the ranks (slab decomposition)
-  for (int ax = 0; ax < 2; ax++) sp->P[ax] = roundup(std::max(sp->b[ax].rows_phys, sp->b[ax].rows_ortho), 4 * ctx->nranks);
+  for (int ax = 0; ax < 2; ax++) sp->P[ax] = roundup(sp->b[ax].lane_rows(), 4 * ctx->nranks);
   r = make_cfg(sp->b[1], sp->P[1], sp->P[0], &sp->cfg[0], ctx->nranks);
   if (r == B2_OK) r = make_cfg(sp->b[0], sp->P[0], sp->P[1], &sp->cfg[1], ctx->nranks);
   if (r == B2_OK) r = sp->b[1].init(sp->cfg[0].C, sp->cfg[0].TPL, sp->cfg[0].fft);   // cfg[0]: lanes along axis 1
@@ -1612,10 +1686,10 @@ int b2_space_destroy(b2_space* sp) {
 int b2_space_shape(const b2_space* sp, int shape_kind, int* rows, int* cols, int* is_complex) {
   int r, c;
   RET(shape_of(sp, shape_kind, &r, &c));
-  bool cx = shape_complex(sp, shape_kind);
-  if (rows) *rows = cx ? r / 2 : r;
-  if (cols) *cols = c;
-  if (is_complex) *is_complex = cx;
+  const int pa = pair_axis(sp, shape_kind);
+  if (rows) *rows = pa == 0 ? r / 2 : r;
+  if (cols) *cols = pa == 1 ? c / 2 : c;
+  if (is_complex) *is_complex = pa >= 0;
   return B2_OK;
 }
 int b2_space_coords(const b2_space* sp, int axis, double* x) {
@@ -1668,7 +1742,7 @@ static int array_copy(const b2_array* a, void* buf, size_t bytes, int to_device)
   }
   double* stage = ctx->stage;
   cudaStream_t st = sp->ctx->stream;
-  const int cx = shape_complex(sp, a->shape_kind);
+  const int cx = pair_axis(sp, a->shape_kind) == 0;   // pairs along axis 1 are already row-major complex
   const size_t total = (size_t)r * c;
   const int grid = (int)((total + 255) / 256);
   if (to_device) {
@@ -1688,7 +1762,7 @@ int b2_array_local_rows(const b2_array* a, int* row_start, int* row_count) {
   int r, c, row0, cnt;
   RET(shape_of(a->sp, a->shape_kind, &r, &c));
   local_rows(a->sp, r, &row0, &cnt);
-  const int div = shape_complex(a->sp, a->shape_kind) ? 2 : 1;
+  const int div = pair_axis(a->sp, a->shape_kind) == 0 ? 2 : 1;
   if (row_start) *row_start = row0 / div;
   if (row_count) *row_count = cnt / div;
   return B2_OK;

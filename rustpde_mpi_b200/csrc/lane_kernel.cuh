@@ -63,6 +63,11 @@ enum LaneOpCode {
   OP_PDMA = 17,    // PdmaPlus2 solve (7 diagonals -2..+4, src/solver/pdma_plus2.rs:123-157): i0 = n, i1 = pitch L of the packed LU
                    //   p0 = [l2 shifted | ka | 1/mu | al | be | ga | de], each L doubles
   OP_CFFT = 19,    // Fourier c2c, n complex points = the lane's 2n reals, modes in FFT order; i0 = n, i1: 0 fwd 1 bwd   p0=tw
+  // split c2c lanes (doubly periodic spaces, see op_split): lanes 2j, 2j + 1 of a CTA hold Re and Im of one complex sequence
+  OP_CPAIR = 20,   // i1 = 0: after OP_RFFT of both lanes, their n-point complex FFT in element order; i1 = 1: the inverse, before
+                   //   OP_RFFT mode 1; i0 = n
+  OP_SDIFF = 21,   // element k (wavenumber k, or k - n for 2k >= n) of a lane pair: (re, im) *= (i k)^{i1} * a,  i0 = n
+  OP_DIAG2 = 22,   // W[lane][e] /= p0[e] + p1[lane] for e < i0 and global lane index < i1
 };
 enum { LD_ACC = 1, LD_PLAIN = 2, LD_MUL = 4, LD_STENCIL = 8,   // LD_STENCIL: value = src[j] + s_{j-2} src[j-2], 2 <= j < len (= n)
        LD_TMA = 16,          // set by the launcher: the slab streams through the warps' staging slots (load_warps)
@@ -1189,6 +1194,83 @@ __device__ __noinline__ void op_cfft(const LaneProg& P, const LaneOp& op, double
   __syncthreads();
 }
 
+// Split c2c lanes: the FourierC2c axis 0 of a doubly periodic space (c2c x r2c).  Along axis 0 the lane index is the axis-1 real
+// column 2j + r, so lane 2j holds Re and lane 2j + 1 Im of one complex sequence over x; both lanes are in one CTA (lane groups of 4
+// or 2) on neighbouring threads (lane = tid % LN).  Each lane runs the real FFT (OP_RFFT) on its own; OP_CPAIR turns the two
+// half spectra into the complex one and back (two-for-one real FFT, z = a + i b):
+//   i1 = 0:  pairs k <= n/2 hold A_k (Re lane) and B_k (Im lane); element k of the Re / Im lane becomes Re / Im of
+//            Z_k = A_k + i B_k, and Z_{n-k} = conj(A_k) + i conj(B_k); elements >= n are cleared
+//   i1 = 1:  the inverse: pair k (k <= n/2) of the Re lane becomes A_k = (Z_k + conj Z_{n-k}) / 2, of the Im lane
+//            B_k = (Z_k - conj Z_{n-k}) / (2i), Z_n = Z_0; A_0, A_{n/2}, B_0, B_{n/2} come out real; elements >= n + 2 are cleared
+// Every element moves between positions k and 2k and between the two lanes, so all of them are read before any is written.
+// OP_SDIFF: thread l of a lane pair takes the elements k = q + (2t + l % 2) TPL of both lanes, so every (Re, Im) element pair is
+// read and written by one thread.  OP_DIAG2 (Poisson / Hholtz with both axes Fourier): one division per mode, by the element's
+// eigenvalue along the lane plus the lane's.
+// The three ops share one non-inlined function, called from lane_kernel's default branch: a call site of its own changes the
+// registers and spills of the generic instances (E = 4), this one leaves every instance as it is without these ops.
+template <int CP, int LN>
+__device__ __noinline__ void op_split(const LaneProg& P, const LaneOp& op, double* __restrict__ W, int g, int lb) {
+  const int TPL = P.TPL, LP = P.LP;
+  const int l = threadIdx.x & (LN - 1), q = threadIdx.x >> Lay<LN>::LOG;
+  const int n = op.i0, im = l & 1;
+  double* wr = W + 4 * (l & ~1);   // the Re lane of this thread's pair
+  double* wi = wr + 4;             // the Im lane
+  if (op.code == OP_CPAIR) {
+    double y[2 * CP];
+#pragma unroll
+    for (int i = 0; i < 2 * CP; i++) {
+      const int e = q + i * TPL;
+      double v = 0.0;
+      if (op.i1 == 0) {
+        if (e < n) {
+          const bool lo = 2 * e <= n;
+          const int k = lo ? e : n - e;
+          const double s = lo ? 1.0 : -1.0;   // -1: conj(A_k), conj(B_k)
+          v = im ? fma(s, wr[Lay<LN>::eix(2 * k + 1)], wi[Lay<LN>::eix(2 * k)])     // Im Z = s Im A + Re B
+                 : fma(-s, wi[Lay<LN>::eix(2 * k + 1)], wr[Lay<LN>::eix(2 * k)]);  // Re Z = Re A - s Im B
+        }
+      } else if (e < n + 2) {
+        const int k = e >> 1, odd = e & 1, m = k ? n - k : 0;
+        const double* z = (im ^ odd) ? wi : wr;
+        const double zk = z[Lay<LN>::eix(k)], zm = z[Lay<LN>::eix(m)];
+        // Re A = (Re Z_k + Re Z_m) / 2, Im A = (Im Z_k - Im Z_m) / 2, Re B = (Im Z_k + Im Z_m) / 2, Im B = (Re Z_m - Re Z_k) / 2
+        v = odd ? (im ? 0.5 * (zm - zk) : 0.5 * (zk - zm)) : 0.5 * (zk + zm);
+      }
+      y[i] = v;
+    }
+    __syncthreads();
+    double* w = W + 4 * l;
+#pragma unroll
+    for (int i = 0; i < 2 * CP; i++) {
+      const int e = q + i * TPL;
+      if (e < LP) w[Lay<LN>::eix(e)] = y[i];
+    }
+  } else if (op.code == OP_SDIFF) {
+    const int d = op.i1 & 3;
+    for (int k = q + im * TPL; k < n; k += 2 * TPL) {
+      const double re = wr[Lay<LN>::eix(k)], mi = wi[Lay<LN>::eix(k)];
+      const double kk = (double)(2 * k >= n ? k - n : k);
+      double f = op.a;
+      for (int t = 0; t < op.i1; t++) f *= kk;
+      double r, s;
+      if (d == 0) { r = re * f; s = mi * f; }
+      else if (d == 1) { r = -mi * f; s = re * f; }
+      else if (d == 2) { r = -re * f; s = -mi * f; }
+      else { r = mi * f; s = -re * f; }
+      wr[Lay<LN>::eix(k)] = r; wi[Lay<LN>::eix(k)] = s;
+    }
+  } else {
+    const int lane = 4 * g + lb + l;
+    if (lane < op.i1) {
+      const double* l0 = (const double*)op.p0;
+      const double mu = ldg((const double*)op.p1 + lane);
+      double* w = W + 4 * l;
+      for (int e = q; e < n; e += TPL) w[Lay<LN>::eix(e)] /= ldg(l0 + e) + mu;
+    }
+  }
+  __syncthreads();
+}
+
 // ChebDirichletNeumann stencil (bc = "hc"): the three-term stencil couples neighbouring elements, so the pair structure of
 // the other banded operators does not apply; element-strided, register-staged (not on any BASELINE configuration's path).
 template <int CP, int LN>
@@ -1410,7 +1492,7 @@ __global__ void B2_LB lane_kernel(const __grid_constant__ LaneProg Pp) {
       case OP_DENSE: op_dense<E + 1, LN>(P, op, W); break;
       case OP_STEN3: op_sten3<E + 1, LN>(P, op, W); break;
       case OP_PDMA: op_pdma<LN>(P, op, W); break;
-      default: op_pointwise<LN>(P, op, W, g, lb); break;
+      default: if (op.code >= OP_CPAIR) op_split<E + 1, LN>(P, op, W, g, lb); else op_pointwise<LN>(P, op, W, g, lb); break;
     }
     if (P.prof && threadIdx.x == 0) {
       atomicAdd(P.prof + op.code, (unsigned long long)(clock64() - t0));
