@@ -27,6 +27,7 @@ typedef struct b2_field b2_field;
 typedef struct b2_array b2_array;
 typedef struct b2_solver b2_solver;
 typedef struct b2_navier b2_navier;
+typedef struct b2_sh2d b2_sh2d;
 
 /* BaseKind enum order of src/field.rs:173-177 (funspace BaseKind) */
 enum b2_base_kind {
@@ -154,6 +155,16 @@ int b2_navier_set_mode(b2_navier* nav, int mode);            /* bit0: fused sche
 int b2_navier_info(const b2_navier* nv, long long* out8);
 int b2_navier_launch_count(const b2_navier* nav, long long* kernels_per_step);
 int b2_navier_poisson_matrices(b2_navier* nav, double* a0, double* cmat0, int* m0);
+
+/* ---- SwiftHohenberg2D (examples/swift_hohenberg_2d.rs): du/dt = [r - (lap + 1)^2] u - u^3, implicit linear part, on a
+ *      caller-owned field of a fourier_c2c x fourier_r2c space.  The object keeps a reference to theta, which must outlive it;
+ *      every step reads and writes theta's vhat on the device (4 lane passes, no host copy). ---- */
+int b2_sh2d_create(b2_field* theta, double r, double dt, const double* scale /* 2 values: Lx, Ly */, b2_sh2d** out); /* swift_hohenberg_2d.rs:54-85 */
+int b2_sh2d_destroy(b2_sh2d* sh);
+int b2_sh2d_update(b2_sh2d* sh, int nsteps);                 /* update_implicit + time += dt, :280-302, :306-311 */
+int b2_sh2d_get_time(const b2_sh2d* sh, double* t);
+int b2_sh2d_set_time(b2_sh2d* sh, double t);
+int b2_sh2d_launch_count(const b2_sh2d* sh, long long* kernels_per_step);
 
 #ifdef __cplusplus
 }

@@ -80,6 +80,12 @@ SYMBOLS = {
     "b2_navier_launch_count": (_I, [_P, C.POINTER(C.c_longlong)]),
     "b2_navier_info": (_I, [_P, C.POINTER(C.c_longlong)]),
     "b2_navier_poisson_matrices": (_I, [_P, _DP, _DP, _IP]),
+    "b2_sh2d_create": (_I, [_P, _D, _D, _DP, _PP]),
+    "b2_sh2d_destroy": (_I, [_P]),
+    "b2_sh2d_update": (_I, [_P, _I]),
+    "b2_sh2d_get_time": (_I, [_P, _DP]),
+    "b2_sh2d_set_time": (_I, [_P, _D]),
+    "b2_sh2d_launch_count": (_I, [_P, C.POINTER(C.c_longlong)]),
 }
 
 _lib = None

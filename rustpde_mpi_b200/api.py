@@ -966,6 +966,138 @@ class _BorrowedSpace(Space2):
         return out
 
 
+class SwiftHohenberg2D:
+    """``SwiftHohenberg2D`` of the reference's examples/swift_hohenberg_2d.rs: ``du/dt = [r - (lap + 1)^2] u - u^3`` on a doubly
+    periodic space ``fourier_c2c(nx) x fourier_r2c(ny)``, the linear part implicit (``update_implicit``, :280-302).  ``update()``
+    runs entirely on the device; ``integrate()``, ``callback()`` and ``exit()`` work as for ``Navier2D``.  ``length``: one length
+    for both axes, as the example (``scale = [length, length]``), or an ``(Lx, Ly)`` pair."""
+
+    io_dir = None   # set to a directory (the reference uses "data") to make callback() write flow files there
+
+    def __init__(self, nx, ny, r, dt, length, ctx=None, init_random=True, seed=0):
+        self.nx, self.ny, self.r, self.dt = nx, ny, float(r), float(dt)
+        self.scale = [float(v) for v in length] if np.ndim(length) else [float(length)] * 2
+        if len(self.scale) != 2:
+            raise B2Error("length: a float or an (Lx, Ly) pair")
+        self.space = Space2(fourier_c2c(nx), fourier_r2c(ny), ctx)
+        self.ctx = self.space.ctx
+        self.theta = Field2(self.space)
+        self._h = C.c_void_p()
+        check(lib().b2_sh2d_create(self.theta._h, self.r, self.dt, (C.c_double * 2)(*self.scale), C.byref(self._h)))
+        if init_random:
+            self.init_random(0.1, seed)   # swift_hohenberg_2d.rs:62
+
+    def close(self):
+        """Free the step's work arrays, then theta and its space."""
+        if getattr(self, "_h", None):
+            _release(lib().b2_sh2d_destroy, self._h)
+            self._h = None
+            self.theta.close()
+            self.space.close()
+
+    __del__ = close
+
+    # initial conditions (swift_hohenberg_2d.rs:187-214)
+    def init_random(self, amp, seed=0):
+        """U(-amp, amp) physical values, then forward.  With several ranks every rank draws the same global array and keeps its
+        rows."""
+        full = np.random.default_rng(seed).uniform(-amp, amp, size=(self.nx, self.ny))
+        self.theta.v = full[self.theta.local_slice(PHYSICAL)]
+        self.theta.forward()
+
+    def init_cos(self, amp, kx, ky):
+        """amp cos(x / length kx pi) cos(y / height ky pi), length and height the coordinate spans, then forward."""
+        x, y = self.theta.x
+        fx = np.cos(x / (x[-1] - x[0]) * kx * np.pi)
+        fy = np.cos(y / (y[-1] - y[0]) * ky * np.pi)
+        self.theta.v = (amp * np.outer(fx, fy))[self.theta.local_slice(PHYSICAL)]
+        self.theta.forward()
+
+    # Integrate (swift_hohenberg_2d.rs:304-345)
+    def update(self, nsteps=1):
+        check(lib().b2_sh2d_update(self._h, int(nsteps)))
+
+    def get_time(self):
+        t = C.c_double()
+        check(lib().b2_sh2d_get_time(self._h, C.byref(t)))
+        return t.value
+
+    def get_dt(self):
+        return self.dt
+
+    def set_time(self, t):
+        check(lib().b2_sh2d_set_time(self._h, float(t)))
+
+    def launches_per_step(self):
+        k = C.c_longlong()
+        check(lib().b2_sh2d_launch_count(self._h, C.byref(k)))
+        return k.value
+
+    def norm(self):
+        """``norm_l2_c64(theta_hat)``: sqrt(sum |theta_hat|^2) / (nx (ny/2 + 1)), reduced on the device (global on several ranks)."""
+        arr = C.c_void_p()
+        check(lib().b2_field_array(self.theta._h, 1, C.byref(arr)))
+        v = C.c_double()
+        check(lib().b2_array_norm2(arr, C.byref(v)))
+        return v.value / (self.nx * (self.ny // 2 + 1))
+
+    def exit(self):
+        """Stop on a NaN in theta_hat: a NaN anywhere makes the norm NaN."""
+        return bool(np.isnan(self.norm()))
+
+    def callback(self):
+        """Print the time and |F|; with ``io_dir`` set, also write ``<io_dir>/flow{time:0>8.2}`` (``.h5`` with h5py, else ``.npz``)."""
+        t = self.get_time()
+        if self.ctx.rank == 0:
+            print(f"Time = {t:6.2e}")
+        if self.io_dir is not None:
+            from . import snapshot as sn
+
+            if self.ctx.rank == 0:
+                os.makedirs(self.io_dir, exist_ok=True)
+            fname = os.path.join(self.io_dir, f"flow{t:0>8.2f}{sn.default_ext()}")
+            try:
+                self.write(fname)
+                if self.ctx.rank == 0:
+                    print(f" ==> {fname!r}")
+            except Exception:  # noqa: BLE001 - swift_hohenberg_2d.rs write() prints and carries on
+                print(f"Error while writing file {fname!r}.")
+        nrm = self.norm()
+        if self.ctx.rank == 0:
+            print(f"|F| = {nrm:6.2e}")
+
+    def write(self, filename):
+        """``_write``: theta.backward(), then the group ``temp`` (``x, dx, y, dy, v, vhat_re, vhat_im``) and the scalars ``time``,
+        ``dt`` and ``r``.  With several ranks the arrays are gathered and rank 0 writes."""
+        from . import snapshot as sn
+
+        f = self.theta
+        f.backward()
+        v, vhat = f.v, f.vhat
+        if self.ctx.nranks > 1:
+            v, vhat = self.ctx.all_gather_rows(v), self.ctx.all_gather_rows(vhat)
+        data = sn.field_datasets("temp", f.x[0], f.x[1], v, vhat)
+        data.update({"time": self.get_time(), "dt": self.dt, "r": self.r})
+        if self.ctx.rank == 0:
+            sn.save_datasets(filename, data)
+        if self.ctx.nranks > 1:
+            self.ctx.barrier()
+
+    def read(self, filename):
+        """Restart from a snapshot of ``write``: theta_hat from ``temp/vhat_re``, ``temp/vhat_im``, then backward(), and the time.
+        A snapshot of another resolution is refused (the low-block copy of ``interpolate_2d`` does not fit FFT-ordered x modes)."""
+        from . import snapshot as sn
+
+        data = sn.load_datasets(filename)
+        vh = data["temp/vhat_re"] + 1j * data["temp/vhat_im"]
+        want = (self.nx, self.ny // 2 + 1)
+        if vh.shape != want:
+            raise B2Error(f"SwiftHohenberg2D.read: snapshot spectrum has shape {vh.shape}, this grid needs {want}")
+        self.theta.vhat = vh[self.theta.local_slice(SPECTRAL)]
+        self.theta.backward()
+        self.set_time(float(data["time"]))
+
+
 MAX_TIMESTEP = 10_000_000
 
 

@@ -740,6 +740,12 @@ struct Prog {
   void fdiff(int modes, int d, double scale, int wrap = 0) { LaneOp* o = add(OP_FDIFF); o->i0 = modes; o->i1 = d; o->a = scale; o->i2 = wrap; }
   void sdiff(int n, int d, double scale) { LaneOp* o = add(OP_SDIFF); o->i0 = n; o->i1 = d; o->a = scale; }
   void diag2(int n, int lanes, const double* lam, const double* mu) { LaneOp* o = add(OP_DIAG2); o->i0 = n; o->i1 = lanes; o->p0 = lam; o->p1 = mu; }
+  // W /= b + a (lam[e] + mu[lane])^2: the implicit Swift-Hohenberg operator of a doubly periodic space
+  void diag2_sq(int n, int lanes, const double* lam, const double* mu, double a, double b) {
+    diag2(n, lanes, lam, mu); LaneOp* o = &p.ops[p.nops - 1]; o->i2 = 1; o->a = a; o->b = b;
+  }
+  void cube(int n, double a) { LaneOp* o = add(OP_CUBE); o->i0 = n; o->a = a; }
+  void hfix(int n) { LaneOp* o = add(OP_HFIX); o->i0 = n; }
   void scalevec(int len, const double* v, int shift) { LaneOp* o = add(OP_SCALEVEC); o->i0 = len; o->i1 = shift; o->p0 = v; }
   void zerotail(int from) { LaneOp* o = add(OP_ZEROTAIL); o->i0 = from; }
   void lanemask(int from) { LaneOp* o = add(OP_LANEMASK); o->i0 = from; }
@@ -1504,6 +1510,45 @@ struct b2_navier {
 #endif
   int use_graph = 1, warm_steps = 0;
 };
+
+// ------------------------------------------------------------------------------------------------
+// SwiftHohenberg2D (examples/swift_hohenberg_2d.rs): update_implicit on a doubly periodic space in four lane passes
+// ------------------------------------------------------------------------------------------------
+struct b2_sh2d {
+  b2_field* theta = nullptr;   // caller-owned; every step reads and writes theta->vhat
+  double r = 0, dt = 0, time = 0;
+  double *A = nullptr, *B = nullptr, *C = nullptr;   // theta_hat x-lane oriented / backward along x / forward along y of the cube
+  DVecD lam, mu;               // 1 - (kx / Lx)^2 per element along x (FFT order), -(ky / Ly)^2 per lane (real column 2 ky + r)
+  long long launches_per_step = 0;
+  int warm_steps = 0;
+#ifndef B2_EMU
+  cudaGraphExec_t graph = nullptr;
+#endif
+};
+
+// One update_implicit (swift_hohenberg_2d.rs:280-302):  theta_hat = (theta_hat - dt F(B(theta_hat)^3)) / matl, mode (0, 0) = 0,
+// column ky = 0 made Hermitian.  The x inverse comes first (as op_backward of a doubly periodic space), so a transpose-only pass
+// brings theta_hat into the x-lane orientation (A); A is read again by the last pass, which adds it to the forward transform.
+static int sh_step(b2_sh2d* sh) {
+  b2_space* sp = sh->theta->sp;
+  const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
+  double* th = sh->theta->vhat->d;
+  Prog p1(sp, 0); p1.load(th, b1.rows_spec); p1.store(sh->A, b1.rows_spec, ST_TRANS);
+  RET(run_pass(p1));
+  Prog p2(sp, 1); p2.load(sh->A, b0.rows_spec); int l = p2.backward_ortho(b0); p2.store(sh->B, l, ST_TRANS);
+  RET(run_pass(p2));
+  // physical values exist only in shared memory: c2r, -dt u^3, r2c along y in one pass
+  Prog p3(sp, 0); p3.load(sh->B, b1.rows_ortho); p3.backward_ortho(b1); p3.cube(b1.rows_phys, -sh->dt); l = p3.forward_ortho(b1);
+  p3.store(sh->C, l, ST_TRANS);
+  RET(run_pass(p3));
+  Prog p4(sp, 1); p4.load(sh->C, b0.rows_phys); p4.forward_ortho(b0); p4.load(sh->A, b0.rows_spec, 1.0, LD_ACC);
+  p4.diag2_sq(b0.m, b1.rows_spec, sh->lam.d, sh->mu.d, sh->dt, 1.0 - sh->r * sh->dt);
+  p4.hfix(b0.n);
+  p4.store(th, b0.rows_spec, ST_TRANS);
+  RET(run_pass(p4));
+  sh->time += sh->dt;
+  return B2_OK;
+}
 
 #ifndef B2_EMU
 static int b2_heap_malloc(void** p, size_t bytes) { CK(cudaMalloc(p, bytes)); return B2_OK; }
@@ -2398,6 +2443,97 @@ int b2_navier_poisson_matrices(b2_navier* nv, double* a0, double* cmat0, int* m0
   if (m0) *m0 = nv->sp_pseu->b[0].m;
   if (!a0 || !cmat0) return B2_OK;
   return b2_poisson_axis0_matrices(nv->pseu, 1.0 / (nv->scale[0] * nv->scale[0]), a0, cmat0);
+}
+
+// ---------------------------------------------------------------------------------------------
+// SwiftHohenberg2D
+// ---------------------------------------------------------------------------------------------
+int b2_sh2d_create(b2_field* theta, double r, double dt, const double* scale, b2_sh2d** out) {
+  if (!theta || !scale || !out) return fail(B2_ERR_ARG, "b2_sh2d_create: null");
+  b2_space* sp = theta->sp;
+  const Base1& b0 = sp->b[0]; const Base1& b1 = sp->b[1];
+  if (!b0.split) return fail(B2_ERR_ARG, "SwiftHohenberg2D needs a fourier_c2c x fourier_r2c space");
+  if (!sp->transforms_ok) return fail(B2_ERR_UNSUPPORTED, "SwiftHohenberg2D: transform size not supported on this space");
+  if (!std::isfinite(r) || !std::isfinite(dt)) return fail(B2_ERR_ARG, "SwiftHohenberg2D: r and dt must be finite");
+  if (!(scale[0] > 0) || !(scale[1] > 0) || !std::isfinite(scale[0]) || !std::isfinite(scale[1]))
+    return fail(B2_ERR_ARG, "SwiftHohenberg2D: lengths must be positive and finite");
+  CK(cudaSetDevice(sp->ctx->device));
+  b2_sh2d* sh = new b2_sh2d();
+  sh->theta = theta; sh->r = r; sh->dt = dt;
+  // matl = 1 - r dt + dt (1 - (kx / Lx)^2 - (ky / Ly)^2)^2 (swift_hohenberg_2d.rs:66-76, integer wavenumbers divided by the lengths)
+  std::vector<double> lam(b0.m), mu(b1.rows_spec);
+  for (int e = 0; e < b0.m; e++) {
+    const double kx = (2 * e < b0.n ? e : e - b0.n) / scale[0];
+    lam[e] = 1.0 - kx * kx;
+  }
+  for (int k = 0; k < b1.m; k++) { const double ky = k / scale[1]; mu[2 * k] = mu[2 * k + 1] = -(ky * ky); }
+  int rc = sh->lam.upload(lam);
+  if (rc == B2_OK) rc = sh->mu.upload(mu);
+  for (double** w : {&sh->A, &sh->B, &sh->C}) if (rc == B2_OK) rc = alloc_zero(sp, w);
+  if (rc != B2_OK) { b2_sh2d_destroy(sh); return rc; }
+  *out = sh;
+  return B2_OK;
+}
+int b2_sh2d_destroy(b2_sh2d* sh) {
+  if (!sh) return B2_OK;
+  b2_ctx* ctx = sh->theta->sp->ctx;
+  for (double* w : {sh->A, sh->B, sh->C}) if (w) ctx_free(ctx, w);
+  sh->lam.release(); sh->mu.release();
+#ifndef B2_EMU
+  if (sh->graph) cudaGraphExecDestroy(sh->graph);
+#endif
+  delete sh;
+  return B2_OK;
+}
+int b2_sh2d_update(b2_sh2d* sh, int nsteps) {
+  if (!sh) return fail(B2_ERR_ARG, "b2_sh2d_update: null handle");
+  if (nsteps < 0) return fail(B2_ERR_ARG, "b2_sh2d_update: nsteps < 0");
+  b2_ctx* ctx = sh->theta->sp->ctx;
+  CK(cudaSetDevice(ctx->device));
+  for (int s = 0; s < nsteps; s++) {
+#ifndef B2_EMU
+    // a fixed launch sequence on fixed arrays: after one direct step, capture one step into a CUDA graph and replay it
+    if (!ctx->d_prof && sh->warm_steps >= 1) {
+      if (!sh->graph) {
+        cudaGraph_t g = nullptr;
+        const long long l0 = ctx->launches;
+        const double t0 = sh->time;
+        CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
+        int r = sh_step(sh);
+        cudaError_t e = cudaStreamEndCapture(ctx->stream, &g);
+        ctx->launches = l0; sh->time = t0;
+        if (r != B2_OK) return r;
+        CK(e);
+        CK(cudaGraphInstantiate(&sh->graph, g, 0));
+        CK(cudaGraphDestroy(g));
+      }
+      CK(cudaGraphLaunch(sh->graph, ctx->stream));
+      ctx->launches += sh->launches_per_step;
+      sh->time += sh->dt;
+      continue;
+    }
+#endif
+    const long long l0 = ctx->launches;
+    RET(sh_step(sh));
+    sh->launches_per_step = ctx->launches - l0;
+    sh->warm_steps++;
+  }
+  return B2_OK;
+}
+int b2_sh2d_get_time(const b2_sh2d* sh, double* t) {
+  if (!sh || !t) return fail(B2_ERR_ARG, "b2_sh2d_get_time: null");
+  *t = sh->time;
+  return B2_OK;
+}
+int b2_sh2d_set_time(b2_sh2d* sh, double t) {
+  if (!sh) return fail(B2_ERR_ARG, "b2_sh2d_set_time: null handle");
+  sh->time = t;
+  return B2_OK;
+}
+int b2_sh2d_launch_count(const b2_sh2d* sh, long long* k) {
+  if (!sh || !k) return fail(B2_ERR_ARG, "b2_sh2d_launch_count: null");
+  *k = sh->launches_per_step;
+  return B2_OK;
 }
 
 }  // extern "C"

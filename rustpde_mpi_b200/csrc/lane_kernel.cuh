@@ -67,7 +67,9 @@ enum LaneOpCode {
   OP_CPAIR = 20,   // i1 = 0: after OP_RFFT of both lanes, their n-point complex FFT in element order; i1 = 1: the inverse, before
                    //   OP_RFFT mode 1; i0 = n
   OP_SDIFF = 21,   // element k (wavenumber k, or k - n for 2k >= n) of a lane pair: (re, im) *= (i k)^{i1} * a,  i0 = n
-  OP_DIAG2 = 22,   // W[lane][e] /= p0[e] + p1[lane] for e < i0 and global lane index < i1
+  OP_DIAG2 = 22,   // W[lane][e] /= s for e < i0 and global lane index < i1, s = p0[e] + p1[lane];  i2 = 1: s = b + a (p0[e] + p1[lane])^2
+  OP_CUBE = 23,    // W[e] = a * W[e]^3 for e < i0, every lane (physical values)
+  OP_HFIX = 24,    // lanes 0, 1 (Re, Im of column ky = 0 along x): element 0 = 0, element n - i = conj(element i) for 1 <= i <= (n-1)/2, n = i0
 };
 enum { LD_ACC = 1, LD_PLAIN = 2, LD_MUL = 4, LD_STENCIL = 8,   // LD_STENCIL: value = src[j] + s_{j-2} src[j-2], 2 <= j < len (= n)
        LD_TMA = 16,          // set by the launcher: the slab streams through the warps' staging slots (load_warps)
@@ -1205,8 +1207,9 @@ __device__ __noinline__ void op_cfft(const LaneProg& P, const LaneOp& op, double
 // Every element moves between positions k and 2k and between the two lanes, so all of them are read before any is written.
 // OP_SDIFF: thread l of a lane pair takes the elements k = q + (2t + l % 2) TPL of both lanes, so every (Re, Im) element pair is
 // read and written by one thread.  OP_DIAG2 (Poisson / Hholtz with both axes Fourier): one division per mode, by the element's
-// eigenvalue along the lane plus the lane's.
-// The three ops share one non-inlined function, called from lane_kernel's default branch: a call site of its own changes the
+// eigenvalue along the lane plus the lane's (mode 1: the Swift-Hohenberg operator b + a (...)^2).  OP_CUBE and OP_HFIX are the
+// other two steps of the Swift-Hohenberg update (b2_sh2d).
+// These ops share one non-inlined function, called from lane_kernel's default branch: a call site of its own changes the
 // registers and spills of the generic instances (E = 4), this one leaves every instance as it is without these ops.
 template <int CP, int LN>
 __device__ __noinline__ void op_split(const LaneProg& P, const LaneOp& op, double* __restrict__ W, int g, int lb) {
@@ -1259,13 +1262,30 @@ __device__ __noinline__ void op_split(const LaneProg& P, const LaneOp& op, doubl
       else { r = mi * f; s = -re * f; }
       wr[Lay<LN>::eix(k)] = r; wi[Lay<LN>::eix(k)] = s;
     }
-  } else {
+  } else if (op.code == OP_DIAG2) {
     const int lane = 4 * g + lb + l;
     if (lane < op.i1) {
       const double* l0 = (const double*)op.p0;
       const double mu = ldg((const double*)op.p1 + lane);
       double* w = W + 4 * l;
-      for (int e = q; e < n; e += TPL) w[Lay<LN>::eix(e)] /= ldg(l0 + e) + mu;
+      for (int e = q; e < n; e += TPL) {
+        const double s = ldg(l0 + e) + mu;
+        w[Lay<LN>::eix(e)] /= op.i2 ? fma(op.a, s * s, op.b) : s;
+      }
+    }
+  } else if (op.code == OP_CUBE) {
+    double* w = W + 4 * l;
+    for (int e = q; e < n; e += TPL) {
+      const double v = w[Lay<LN>::eix(e)];
+      w[Lay<LN>::eix(e)] = op.a * (v * v * v);
+    }
+  } else if (g == 0 && lb == 0 && l < 2) {   // OP_HFIX: the CTA that holds lanes 0 and 1 of group 0 (LN = 2 splits the group)
+    // the elements read (1 .. (n-1)/2) and written (0 and n - (n-1)/2 .. n - 1) are disjoint, so no barrier in between
+    double* w = W + 4 * l;
+    const double s = l ? -1.0 : 1.0;
+    for (int e = q; e < n; e += TPL) {
+      if (e == 0) w[0] = 0.0;
+      else if (2 * e > n) w[Lay<LN>::eix(e)] = s * w[Lay<LN>::eix(n - e)];
     }
   }
   __syncthreads();
